@@ -276,11 +276,7 @@ int env_int(const char* name, int dflt) {
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // smallest f32 >= thr, so that (m >= thr_f) in f32 equals ((double)m >= thr) for every f32 m
-float threshold_f32(double thr) {
-  float t = (float)thr;
-  if ((double)t < thr) t = nextafterf(t, INFINITY);
-  return t;
-}
+float threshold_f32(double thr) { return gpr::text::threshold_up(thr); }
 
 bool power_truthy(double thr) { return thr != 0.0 && !std::isnan(thr); }
 
@@ -1736,6 +1732,7 @@ int gpr_text_parse(gpr_ctx* ctx, int32_t slot, gpr_text_span* spans, uint32_t n_
   // the device works in milliseconds, the resolution of Prometheus timestamps
   g.t_end = grid->t_end * 1000, g.t_lo = (grid->t_end - grid->window_seconds) * 1000;
   g.step = (uint32_t)(grid->step * 1000), g.T = n_samples;
+  g.power = gpr::text::power_snap(plane == 1 ? grid->power_threshold : 0.0);
   if (resident) {
     if (!ctx->d_res_util) return fail(ctx, GPR_E_STATE, "no resident window (gpr_resident_init)");
     if (n_samples != ctx->res_T || (uint64_t)n_rows > (uint64_t)ctx->res_P * ctx->res_G)

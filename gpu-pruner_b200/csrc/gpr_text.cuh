@@ -77,6 +77,11 @@ struct Span {        // mirrors gpr_text_span (include/gpr.h)
 //     col  = (col_end - back) mod T
 // A dense window has col_end = T - 1 (column c = bucket T-1-c); the resident ring of daemon mode passes
 // the ring position of its newest bucket.
+struct PowerSnap {   // how power samples are stored against the veto threshold: power_snap() / snap_power() below
+  double thr;        // NaN = no snapping
+  float up, down;    // smallest f32 >= thr, and the f32 just below it
+};
+
 struct Grid {
   int64_t t_end;     // newest millisecond (inclusive)
   int64_t t_lo;      // t_end - window (exclusive)
@@ -85,6 +90,7 @@ struct Grid {
   uint32_t col_end;  // column of the newest bucket
   uint32_t pad;
   uint64_t ld;       // elements between rows of the plane
+  PowerSnap power;   // power_snap(threshold) for the power plane, power_snap(0) for the util plane
 };
 
 constexpr int64_t kBadTs = INT64_MIN / 4;  // timestamp that is no sane epoch time: outside any window
@@ -217,15 +223,61 @@ GPR_HD uint32_t f32_bits(float f) {
 GPR_HD float quiet_nan_f32() { return f32_from_bits(0x7fc00000u); }
 constexpr uint32_t kFillBits = 0xFFFFFFFFu;  // "no sample": a NaN that is -1 as an int (below every non-negative value)
 
+// ---- power samples against the veto threshold ------------------------------------------------------------
+// The veto compares the f32 row max with up = the smallest f32 >= thr (gpr_decide), which equals Prometheus'
+// float64 `x >= thr` only for samples that are f32 already: a reading within half an f32 ulp below thr
+// (149.999999 for 150) rounds UP to `up` and would veto.  So power samples are stored snapped:
+//     x >= thr  ->  at least up          x < thr  ->  at most down, the f32 just below up
+// after which `max >= up` holds exactly when some x >= thr, for every float64 threshold.  NaN and
+// +-Inf are left alone (they compare the same either way); thr = NaN turns the snap off (util plane, or no
+// power clause: a threshold of 0 or NaN, the truthiness rule of the template).  PowerSnap is defined above Grid.
+GPR_HD float f32_next_up(float f) {  // toward +Inf; f is neither NaN nor +Inf
+  const uint32_t b = f32_bits(f);
+  if ((b & 0x7fffffffu) == 0u) return f32_from_bits(1u);
+  return f32_from_bits((b >> 31) ? b - 1u : b + 1u);
+}
+GPR_HD float f32_next_down(float f) {  // toward -Inf; f is neither NaN nor -Inf
+  const uint32_t b = f32_bits(f);
+  if ((b & 0x7fffffffu) == 0u) return f32_from_bits(0x80000001u);
+  return f32_from_bits((b >> 31) ? b + 1u : b - 1u);
+}
+
+// smallest f32 >= thr: (m >= threshold_up(thr)) in f32 equals ((double)m >= thr) for every f32 m
+GPR_HD float threshold_up(double thr) {
+  float t = (float)thr;
+  if ((double)t < thr) t = f32_next_up(t);
+  return t;
+}
+
+GPR_HD PowerSnap power_snap(double thr) {
+  PowerSnap s;
+  if (thr != thr || thr == 0.0) {
+    s.thr = bits_to_double(0x7ff8000000000000ull);
+    s.up = s.down = 0.0f;
+    return s;
+  }
+  s.thr = thr;
+  s.up = threshold_up(thr);
+  s.down = f32_bits(s.up) == 0xff800000u ? s.up : f32_next_down(s.up);  // thr = -Inf: nothing is below it
+  return s;
+}
+
+// x: the sample in float64, f: its f32 (to_f32)
+GPR_HD float snap_power(double x, float f, const PowerSnap& s) {
+  if (x >= s.thr) return f < s.up ? s.up : f;
+  if (x < s.thr && f >= s.up) return s.down;
+  return f;
+}
+
 // ---- one sample ------------------------------------------------------------------------------------------
 // `Src` is anything with `uint8_t operator[](uint32_t) const` (shared-memory tile on the device, a plain
 // buffer in the emulation).  Offsets are relative to the tile; nothing at or beyond p + kMaxSample is read.
 //
 // [-+]digits[.digits][(e|E)[-+]digits] at t[p...] -> *v.  Prometheus prints sample values with strconv 'f' and
 // switches to 'e' below 1e-6 and from 1e21 on (util/jsonutil MarshalFloat), so both forms occur.
-// Returns the offset after the number, 0 = not convertible here.
+// Returns the offset after the number, 0 = not convertible here.  `snap`: power_snap() of the plane (see above).
 template <typename Src>
-GPR_HD uint32_t parse_value(const Src& t, uint32_t p, uint32_t limit, float* val, uint32_t* tiny) {
+GPR_HD uint32_t parse_value(const Src& t, uint32_t p, uint32_t limit, float* val, uint32_t* tiny, const PowerSnap& snap) {
   bool neg = false;
   uint32_t c = t[p];
   if (c == '-' || c == '+') neg = c == '-', c = t[++p];
@@ -279,10 +331,19 @@ GPR_HD uint32_t parse_value(const Src& t, uint32_t p, uint32_t limit, float* val
     } else if (!eisel_lemire(m, e10, &d)) {
       return 0;
     }
+    // (the exact integer and zero paths above need no snap: a sample that is an f32 compares the same either way)
     f = to_f32(d, tiny);
+    *val = snap_power(neg ? -d : d, neg ? -f : f, snap);
+    return p;
   }
   *val = neg ? -f : f;
   return p;
+}
+
+// the same for a plane without a power clause (utilisation, PROF ratios): plain rounding
+template <typename Src>
+GPR_HD uint32_t parse_value(const Src& t, uint32_t p, uint32_t limit, float* val, uint32_t* tiny) {
+  return parse_value(t, p, limit, val, tiny, power_snap(0.0));
 }
 
 // t[p] == '['.  `[digits[.digits],` -> milliseconds.  At most 13 integer and 3 fractional digits (Prometheus
@@ -310,7 +371,7 @@ GPR_HD uint32_t parse_timestamp(const Src& t, uint32_t p, int64_t* ts) {
 
 // Returns the offset after the sample's ']' or 0 (hard).
 template <typename Src>
-GPR_HD uint32_t parse_sample(const Src& t, uint32_t p, int64_t* ts, float* val, uint32_t* tiny) {
+GPR_HD uint32_t parse_sample(const Src& t, uint32_t p, int64_t* ts, float* val, uint32_t* tiny, const PowerSnap& snap) {
   const uint32_t limit = p + kMaxSample - 2;
   uint32_t q = parse_timestamp(t, p, ts);
   if (q == 0 || t[q + 1] != '"') return 0;
@@ -327,7 +388,7 @@ GPR_HD uint32_t parse_sample(const Src& t, uint32_t p, int64_t* ts, float* val, 
     *val = f32_from_bits(neg ? 0xff800000u : 0x7f800000u);
     q += 3;
   } else {
-    q = parse_value(t, q, limit, val, tiny);
+    q = parse_value(t, q, limit, val, tiny, snap);
     if (q == 0) return 0;
   }
   if (t[q] != '"' || t[q + 1] != ']') return 0;
@@ -400,7 +461,7 @@ GPR_HD void parse_candidate(const Src& tile, uint64_t tile_off, uint32_t o, cons
   int64_t ts;
   float v;
   uint32_t tiny = 0;
-  const uint32_t q = parse_sample(tile, o, &ts, &v, &tiny);
+  const uint32_t q = parse_sample(tile, o, &ts, &v, &tiny, g.power);
   // between samples exactly one ',' ; after the last one the list closes at `se`
   if (q == 0 || tile_off + q > se || !(tile_off + q == se || (tile[q] == ',' && tile[q + 1] == '['))) {
     sink.hard(s);

@@ -402,10 +402,11 @@ class IdleEngine:
 
     def text_parse(self, spans: np.ndarray, t_end: int, step: int, T: int, n_rows: int, slot: int = 0,
                    plane: int = 0, fill: bool = True, window_seconds: Optional[int] = None,
-                   resident: bool = False) -> np.ndarray:
+                   resident: bool = False, power_threshold: Optional[float] = 0.0) -> np.ndarray:
         """Parse the samples of ``spans`` (structured array of SPAN_DTYPE, sorted by begin) of the text in
         ``slot`` into the context's plane (or, ``resident=True``, the resident ring); returns the spans with
-        their out-fields filled.  ``window_seconds`` defaults to ``T * step``."""
+        their out-fields filled.  ``window_seconds`` defaults to ``T * step``.  ``power_threshold``: for the
+        power plane, the threshold it will be decided with (samples are snapped to it, include/gpr.h)."""
         spans = np.ascontiguousarray(spans, dtype=self.SPAN_DTYPE)
         g = ffi.gpr_text_grid()
         g.struct_size = C.sizeof(ffi.gpr_text_grid)
@@ -413,6 +414,7 @@ class IdleEngine:
         g.t_end, g.step = int(t_end), int(step)
         g.window_seconds = int(T) * int(step) if window_seconds is None else int(window_seconds)
         g.n_samples, g.n_rows = int(T), int(n_rows)
+        g.power_threshold = 0.0 if power_threshold is None else float(power_threshold)
         self._check(self._lib.gpr_text_parse(self._h, slot, _ptr(spans), len(spans), C.byref(g), plane))
         return spans
 

@@ -74,7 +74,7 @@ class gpr_text_grid(C.Structure):
     _fields_ = [
         ("struct_size", C.c_uint32), ("flags", C.c_uint32),
         ("t_end", C.c_int64), ("window_seconds", C.c_int64), ("step", C.c_int64),
-        ("n_samples", C.c_uint32), ("n_rows", C.c_uint32),
+        ("n_samples", C.c_uint32), ("n_rows", C.c_uint32), ("power_threshold", C.c_double),
     ]
 
 

@@ -85,6 +85,8 @@ GPH_API int gph_format_float(double v, char* out, int cap) { return put(gph::for
 
 // ingest: JSON texts in, tensor out.  Returns 0 or negative; dims written to dims[3] = P,G,T.
 // util_out/power_out may be NULL to query dimensions + the pod table (JSON) first.
+// gph_ingest_for_threshold: the same, with the threshold the power plane will be decided with
+// (IngestOptions::power_threshold: power samples are snapped to it; 0 = none, which is what gph_ingest does).
 static int g_ingest_threads = -1;  // -1: DOM path; >= 0: text path with that many threads (0 = all)
 GPH_API void gph_ingest_mode(int threads) { g_ingest_threads = threads; }
 // response of the `node_dmi_info` query applied by the following gph_ingest calls (NULL / "" = none)
@@ -92,12 +94,12 @@ static std::string g_dmi_json;
 GPH_API void gph_ingest_dmi(const char* dmi_json) { g_dmi_json = dmi_json ? dmi_json : ""; }
 static gph::Window g_last_window;  // the window of the most recent successful gph_ingest (tensor dropped)
 
-GPH_API int gph_ingest(const char* util_json, const char* prof_json, const char* power_json,
-                       long long duration_min, long long step, long long t_end, unsigned* dims,
-                       float* util_out, float* power_out, char* pods_json, int cap) {
+GPH_API int gph_ingest_for_threshold(const char* util_json, const char* prof_json, const char* power_json,
+                                     long long duration_min, long long step, long long t_end, double power_threshold,
+                                     unsigned* dims, float* util_out, float* power_out, char* pods_json, int cap) {
   try {
     gph::IngestOptions o;
-    o.duration_min = duration_min, o.step = step, o.t_end = t_end;
+    o.duration_min = duration_min, o.step = step, o.t_end = t_end, o.power_threshold = power_threshold;
     gph::Window w;
     const auto t0 = std::chrono::steady_clock::now();
     if (g_ingest_threads >= 0) {
@@ -152,6 +154,13 @@ GPH_API int gph_ingest(const char* util_json, const char* prof_json, const char*
     if (pods_json) put(std::string("{\"error\":\"") + gph::json_escape(e.what()) + "\"}", pods_json, cap);
     return -1;
   }
+}
+
+GPH_API int gph_ingest(const char* util_json, const char* prof_json, const char* power_json,
+                       long long duration_min, long long step, long long t_end, unsigned* dims,
+                       float* util_out, float* power_out, char* pods_json, int cap) {
+  return gph_ingest_for_threshold(util_json, prof_json, power_json, duration_min, step, t_end, 0.0, dims, util_out,
+                                  power_out, pods_json, cap);
 }
 
 // Exact `sum by` for the window of the last gph_ingest: corrects the engine's / oracle's raw verdict arrays in

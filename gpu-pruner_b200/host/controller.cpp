@@ -125,6 +125,7 @@ class FileSource : public WindowSource {
     if (want_power && file_exists(d + "/power.json")) power = slurp(d + "/power.json"), ppower = &power;
     IngestOptions opt;
     opt.duration_min = args.duration;
+    opt.power_threshold = want_power ? *args.power_threshold : 0.0;
     if (file_exists(d + "/query.json")) {
       const Json meta = Json::parse_file(d + "/query.json");
       opt.t_end = (int64_t)meta["end"].as_number(0);

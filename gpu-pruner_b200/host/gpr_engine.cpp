@@ -193,6 +193,7 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
     g.flags = (grid.fill ? GPR_TEXT_FILL : 0u) | (grid.resident ? GPR_TEXT_RESIDENT : 0u);
     g.t_end = grid.t_end, g.window_seconds = grid.span, g.step = grid.step;
     g.n_samples = grid.T, g.n_rows = grid.n_rows;
+    g.power_threshold = grid.power_threshold;
     check(gpr_text_parse(ctx_, slot, spans.data(), (uint32_t)spans.size(), &g, plane), "gpr_text_parse");
   }
   void patch_row(int plane, uint32_t row, uint32_t T, const float* data, uint32_t n_newest, bool resident) override {

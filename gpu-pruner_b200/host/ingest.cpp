@@ -91,7 +91,7 @@ Window ingest_matrix(const Json& util, const Json* prof, const Json* power, cons
   if (power) scan(*power, true, false);
   finish_shape(w, opt, newest, vote.result(), power != nullptr);
 
-  auto place = [&](const std::vector<RawSeries>& list, std::vector<float>& plane) {
+  auto place = [&](const std::vector<RawSeries>& list, std::vector<float>& plane, const gpr::text::PowerSnap& snap) {
     for (const RawSeries& rs : list) {
       float* row = plane.data() + ((size_t)rs.pod * w.G + rs.slot) * w.T;
       for (const Json& tv : rs.values->items()) {
@@ -101,12 +101,12 @@ Window ingest_matrix(const Json& util, const Json* prof, const Json* power, cons
           ++w.stats.samples_out_of_window;
           continue;
         }
-        merge_cell(row[col], to_f32(sample_value(tv[1]), &w.stats.tiny_values_clamped));
+        merge_cell(row[col], to_cell(sample_value(tv[1]), snap, &w.stats.tiny_values_clamped));
       }
     }
   };
-  place(useries, w.util);
-  if (power) place(pseries, w.power);
+  place(useries, w.util, gpr::text::power_snap(0.0));
+  if (power) place(pseries, w.power, gpr::text::power_snap(opt.power_threshold));
   return w;
 }
 
@@ -170,7 +170,7 @@ Window ingest_matrix_text(const std::string& util, const std::string* prof, cons
   }
   finish_shape(w, opt, newest, vote.result(), power != nullptr);
 
-  auto place = [&](std::vector<TextSeries>& list, std::vector<float>& plane) {
+  auto place = [&](std::vector<TextSeries>& list, std::vector<float>& plane, const gpr::text::PowerSnap& snap) {
     // rows written by exactly one series can be filled concurrently; shared rows are merged afterwards
     std::vector<uint32_t> writers((size_t)w.P * w.G, 0);
     for (const TextSeries& ts : list) ++writers[(size_t)ts.pod * w.G + ts.slot];
@@ -190,7 +190,7 @@ Window ingest_matrix_text(const std::string& util, const std::string* prof, cons
             ++n_out;
             return;
           }
-          merge_cell(row[col], to_f32(v, &n_tiny));
+          merge_cell(row[col], to_cell(v, snap, &n_tiny));
         });
       }
       IngestStats& s = st[(size_t)tid];
@@ -218,8 +218,8 @@ Window ingest_matrix_text(const std::string& util, const std::string* prof, cons
       w.stats.tiny_values_clamped += s.tiny_values_clamped;
     }
   };
-  place(useries, w.util);
-  if (power) place(pseries, w.power);
+  place(useries, w.util, gpr::text::power_snap(0.0));
+  if (power) place(pseries, w.power, gpr::text::power_snap(opt.power_threshold));
   return w;
 }
 

@@ -98,6 +98,10 @@ struct IngestOptions {
   // what was scraped since the previous tick; the rest of the window is resident in HBM
   int64_t slice_seconds = 0;
   bool resident = false;              // keep the window resident for the following ticks
+  // --power-threshold the power plane will be decided with: its samples are stored snapped to it so that the f32
+  // veto agrees with Prometheus' float64 `x >= threshold` (include/gpr.h, gpr_window.power_threshold).
+  // 0 / NaN = no power clause: plain rounding
+  double power_threshold = 0.0;
 };
 
 // thrown by a delta ingest when the resident state cannot absorb the tick (new GPU slot beyond the ring's shape,

@@ -354,6 +354,7 @@ struct DeviceIngestSession::State {
   bool valid = false;              // the resident ring holds the window ending at w.t_end
   uint32_t pods_cap = 0;           // pods the ring has rows for
   bool with_power = false;
+  double power_threshold = 0.0;    // what the resident power samples are snapped to
   std::vector<std::pair<uint32_t, uint32_t>> prof_rows;  // (pod, slot) fed by PROF series, sorted
 };
 
@@ -388,6 +389,9 @@ Window DeviceIngestSession::ingest(const std::string& util, const std::string* p
     else if (opt.slice_seconds % opt.step != 0) why = "the slice is not a whole number of steps";
     else if (opt.slice_seconds / opt.step >= (int64_t)st.w.T) why = "the slice is as long as the window";
     else if ((power != nullptr) != st.with_power) why = "power plane appeared / disappeared";
+    else if (power && !(opt.power_threshold == st.power_threshold ||
+                        (std::isnan(opt.power_threshold) && std::isnan(st.power_threshold))))
+      why = "the power threshold changed";
     if (why) {
       st.valid = false;
       throw NeedFullWindow(why);
@@ -435,6 +439,7 @@ Window DeviceIngestSession::ingest(const std::string& util, const std::string* p
   if (!delta) {
     finish_shape(w, opt, 0, 1, power != nullptr, /*allocate=*/false);  // t_end / step given: nothing to infer
     st.with_power = power != nullptr;
+    st.power_threshold = opt.power_threshold;
     st.prof_rows = prof_rows;
     if (opt.resident) {
       st.pods_cap = w.P + w.P / 4 + 64;   // head-room: new pods get rows without a rebuild
@@ -493,6 +498,7 @@ Window DeviceIngestSession::ingest(const std::string& util, const std::string* p
       TextDevice::TextGrid grid;
       grid.t_end = w.t_end, grid.span = parse_span, grid.step = w.step, grid.T = w.T, grid.n_rows = n_rows;
       grid.fill = fill, grid.resident = resident;
+      grid.power_threshold = plane == 1 ? opt.power_threshold : 0.0;
       dev_.parse(texts[k]->slot, spans[k], grid, plane);
       rep.parse_ms += ms_since(tp);
       fill = false;
@@ -509,6 +515,7 @@ Window DeviceIngestSession::ingest(const std::string& util, const std::string* p
     std::vector<int64_t> row_slot(any_dirty ? n_rows : 0, -1);
     Window bucket;  // the grid of the patched columns: the newest `patch_cols` buckets
     bucket.t_end = w.t_end, bucket.step = w.step, bucket.span = parse_span, bucket.T = patch_cols;
+    const gpr::text::PowerSnap snap = gpr::text::power_snap(plane == 1 ? opt.power_threshold : 0.0);
     for (size_t k = 0; k < texts.size(); ++k) {
       const std::string& t = *texts[k]->text;
       for (const gpr_text_span& sp : spans[k]) {
@@ -531,7 +538,7 @@ Window DeviceIngestSession::ingest(const std::string& util, const std::string* p
             ++w.stats.samples_out_of_window;
             return;
           }
-          merge_cell(row[col], to_f32(v, &w.stats.tiny_values_clamped));
+          merge_cell(row[col], to_cell(v, snap, &w.stats.tiny_values_clamped));
         });
       }
     }

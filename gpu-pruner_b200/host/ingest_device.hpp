@@ -40,6 +40,7 @@ class TextDevice {
     uint32_t T = 0, n_rows = 0;
     bool fill = true;        // start from an all-"no sample" plane
     bool resident = false;   // destination = the resident ring of daemon mode instead of the context plane
+    double power_threshold = 0.0;  // plane 1: samples are snapped to it (IngestOptions::power_threshold)
   };
   virtual void parse(int slot, std::vector<gpr_text_span>& spans, const TextGrid& grid, int plane) = 0;
   // overwrite the newest `n_newest` buckets of `row` (chronological order in `data`; n_newest == T: the whole

@@ -13,6 +13,7 @@
 #include <unordered_map>
 #include <vector>
 
+#include "../csrc/gpr_text.cuh"  // power_snap / snap_power: one rule for the CPU and the device parser
 #include "ingest.hpp"
 
 namespace gph {
@@ -106,6 +107,12 @@ inline float to_f32(double x, uint64_t* clamped) {
     ++*clamped;
   }
   return f;
+}
+
+// what a cell of a plane holds for sample x: util plane (snap = power_snap(0)) rounded, power plane also snapped to
+// the veto threshold (gpr_text.cuh)
+inline float to_cell(double x, const gpr::text::PowerSnap& snap, uint64_t* clamped) {
+  return gpr::text::snap_power(x, to_f32(x, clamped), snap);
 }
 
 // several samples of one series in one bucket: NaN-aware max — what max_over_time over the row computes anyway

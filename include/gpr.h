@@ -124,7 +124,17 @@ typedef struct gpr_config {
  *   row_stride      elements between consecutive (p,g) rows; 0 means n_samples.
  *   power_threshold watts; the veto clause exists iff power != NULL and the threshold is
  *                   neither 0.0 nor NaN (Jinja truthiness of `args.power_threshold`,
- *                   query.promql.j2:36).  veto(p) = any g: max_t power[p][g][:] >= threshold.
+ *                   query.promql.j2:36).  veto(p) = any g: max_t power[p][g][:] >= up, with
+ *                   up = the smallest f32 >= threshold — exactly `(double)cell >= threshold`.
+ *                   That equals Prometheus' float64 `x >= threshold` on the samples x only if
+ *                   each cell was stored from its sample x by the POWER RULE:
+ *                       f = x rounded to nearest f32;
+ *                       if (x >= threshold && f <  up) f = up;
+ *                       if (x <  threshold && f >= up) f = the f32 just below up;
+ *                   (NaN and +-Inf unchanged).  Plain rounding alone vetoes a reading within
+ *                   half an f32 ulp below the threshold (149.999999 W rounds to 150.0f).
+ *                   gpr_text_parse applies the rule (gpr_text_grid.power_threshold); a caller
+ *                   that fills power planes itself (gpr_decide, gpr_append) must apply it too.
  *   eligible[p]     u8 or NULL: 0 = pod fails the Pending / missing-timestamp gates
  *                   (main.rs:473-492).  NULL = all eligible.
  *   created_ts[p]   i64 or NULL: pod creation time in caller-chosen ticks; the pod is skipped
@@ -207,7 +217,8 @@ GPR_API int gpr_decide_batch_async(gpr_ctx *ctx, const gpr_window *windows, gpr_
  * irrelevant to the verdict.                                                              */
 GPR_API int gpr_resident_init(gpr_ctx *ctx, uint32_t n_pods, uint32_t n_gpus, uint32_t n_samples,
                       uint32_t flags /* GPR_F_POWER_PLANE | GPR_F_BLOCK_INDEX */);
-/* new columns laid out [p][g][n_new] (row_stride 0 = n_new); power_cols may be NULL.      */
+/* new columns laid out [p][g][n_new] (row_stride 0 = n_new); power_cols may be NULL (its
+ * cells stored by the power rule of gpr_window.power_threshold).                          */
 GPR_API int gpr_append(gpr_ctx *ctx, const float *util_cols, const float *power_cols, uint32_t n_new,
                uint64_t row_stride, int32_t mem_kind);
 /* Open the next n_new buckets of the ring without data: their columns become "no sample" in every row of
@@ -346,6 +357,9 @@ typedef struct gpr_text_grid {
   int64_t step;            /* seconds per column, > 0                                               */
   uint32_t n_samples;      /* columns; >= ceil(window_seconds / step)                               */
   uint32_t n_rows;
+  double power_threshold;  /* plane 1: the gpr_window.power_threshold the plane will be decided with;
+                              its samples are stored by the power rule of gpr_window (0.0 / NaN: no
+                              power clause, plain rounding).  Ignored for plane 0.                  */
 } gpr_text_grid;
 #define GPR_TEXT_FILL 1u     /* fill the destination plane with "no sample" first (context planes)    */
 #define GPR_TEXT_RESIDENT 2u /* destination = the resident ring (gpr_resident_init): n_samples must be its

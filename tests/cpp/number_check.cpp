@@ -4,8 +4,10 @@
 //   E <mantissa> <exp10>   ->  "<ok> <hex bits of the binary64>"      eisel_lemire
 //   V <decimal text>       ->  "<consumed> <hex bits of the f32> <tiny>"   parse_value (0 consumed = declined)
 //   T <timestamp text>     ->  "<offset of ','> <seconds>"            parse_timestamp on "[<text>,"
+//   S <threshold> <text>   ->  "<consumed> <hex f32> <hex up> <hex down>"   parse_value into a power plane (power_snap)
 #include <cinttypes>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <string>
 
@@ -42,6 +44,22 @@ int main() {
       uint32_t bits;
       memcpy(&bits, &f, 4);
       printf("%u %08x %u\n", q == len ? q : 0u, q == len ? bits : 0u, tiny);
+    } else if (line[0] == 'S') {
+      // S <threshold> <decimal text>  ->  "<consumed> <hex bits of the stored power sample> <hex up> <hex down>"
+      char* rest = nullptr;
+      const double thr = strtod(line + 2, &rest);
+      while (*rest == ' ') ++rest;
+      uint8_t buf[256] = {0};
+      const size_t len = strlen(rest);
+      memcpy(buf, rest, len);
+      buf[len] = '"';
+      float f = 0;
+      uint32_t tiny = 0;
+      const tx::PowerSnap snap = tx::power_snap(thr);
+      const uint32_t q = tx::parse_value(Buf{buf}, 0, tx::kMaxSample - 2, &f, &tiny, snap);
+      uint32_t bits, up, down;
+      memcpy(&bits, &f, 4), memcpy(&up, &snap.up, 4), memcpy(&down, &snap.down, 4);
+      printf("%u %08x %08x %08x\n", q == len ? q : 0u, q == len ? bits : 0u, up, down);
     } else if (line[0] == 'T') {
       uint8_t buf[256] = {0};
       const size_t len = strlen(line + 2);

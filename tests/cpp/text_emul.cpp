@@ -5,7 +5,7 @@
 // [power.json]) is ingested by the CPU text path and by the emulated device path; shape, pods,
 // statistics and every tensor cell must agree, or both must reject the input.
 //
-//   text_emul <t_end> <step> <duration_min> <case_dir>...
+//   text_emul <t_end> <step> <duration_min> <case_dir>...       (case_dir/power_threshold: optional, one number)
 // prints per case:  OK device=<0|1> spans=.. hard=.. patched=.. [reason]  |  REJECT  |  MISMATCH <what>
 #include <algorithm>
 #include <cmath>
@@ -99,6 +99,7 @@ class EmulDevice : public TextDevice {
     memset(&g, 0, sizeof g);
     g.t_end = grid.t_end * 1000, g.t_lo = (grid.t_end - grid.span) * 1000, g.step = (uint32_t)(grid.step * 1000), g.T = T;
     g.col_end = grid.resident ? (ring_head_ + T - 1) % T : T - 1, g.ld = T;
+    g.power = tx::power_snap(plane == 1 ? grid.power_threshold : 0.0);  // as gpr_text_parse sets it (gpr_api.cu)
     const std::vector<uint8_t>& text = text_[slot];
     const uint64_t n = n_[slot];
     const tx::Span* sp = reinterpret_cast<const tx::Span*>(spans.data());
@@ -355,18 +356,22 @@ int main(int argc, char** argv) {
       continue;
     }
     const bool has_prof = slurp(dir + "/prof.json", &prof), has_power = slurp(dir + "/power.json", &power);
+    // optional: the --power-threshold the power plane is ingested for (its samples are snapped to it)
+    std::string thr_text;
+    IngestOptions oc = o;
+    if (slurp(dir + "/power_threshold", &thr_text)) oc.power_threshold = strtod(thr_text.c_str(), nullptr);
     Window wc, wd;
     bool ok_c = true, ok_d = true;
     std::string err_c, err_d;
     DeviceIngestReport rep;
     EmulDevice dev;
     try {
-      wc = ingest_matrix_text(util, has_prof ? &prof : nullptr, has_power ? &power : nullptr, o, 2);
+      wc = ingest_matrix_text(util, has_prof ? &prof : nullptr, has_power ? &power : nullptr, oc, 2);
     } catch (const std::exception& e) {
       ok_c = false, err_c = e.what();
     }
     try {
-      wd = ingest_matrix_device(dev, util, has_prof ? &prof : nullptr, has_power ? &power : nullptr, o, &rep);
+      wd = ingest_matrix_device(dev, util, has_prof ? &prof : nullptr, has_power ? &power : nullptr, oc, &rep);
     } catch (const std::logic_error& e) {
       printf("MISMATCH %s %s\n", dir.c_str(), e.what());
       ++bad;

@@ -138,21 +138,23 @@ def group_values(series_max):
     return out
 
 
-def ingest(util, prof=None, power=None, duration_min=30, step=0, t_end=0):
+def ingest(util, prof=None, power=None, duration_min=30, step=0, t_end=0, power_threshold=None):
+    """power_threshold: what the power plane will be decided with (its samples are snapped to it; None = none)"""
     import numpy as np
     dims = (C.c_uint * 3)()
     enc = lambda j: None if j is None else json.dumps(j).encode()
+    thr = C.c_double(0.0 if power_threshold is None else float(power_threshold))
     meta = C.create_string_buffer(CAP)
-    rc = lib().gph_ingest(enc(util), enc(prof), enc(power), C.c_longlong(duration_min), C.c_longlong(step),
-                          C.c_longlong(t_end), dims, None, None, meta, CAP)
+    rc = lib().gph_ingest_for_threshold(enc(util), enc(prof), enc(power), C.c_longlong(duration_min),
+                                        C.c_longlong(step), C.c_longlong(t_end), thr, dims, None, None, meta, CAP)
     if rc != 0:
         raise RuntimeError(json.loads(meta.value.decode()).get("error", "ingest failed"))
     P, G, T = dims[0], dims[1], dims[2]
     u = np.zeros((P, G, T), np.float32)
     w = np.zeros((P, G, T), np.float32) if power is not None else None
-    rc = lib().gph_ingest(enc(util), enc(prof), enc(power), C.c_longlong(duration_min), C.c_longlong(step),
-                          C.c_longlong(t_end), dims, u.ctypes.data_as(C.c_void_p),
-                          None if w is None else w.ctypes.data_as(C.c_void_p), meta, CAP)
+    rc = lib().gph_ingest_for_threshold(enc(util), enc(prof), enc(power), C.c_longlong(duration_min),
+                                        C.c_longlong(step), C.c_longlong(t_end), thr, dims, u.ctypes.data_as(C.c_void_p),
+                                        None if w is None else w.ctypes.data_as(C.c_void_p), meta, CAP)
     assert rc == 0
     return u, w, json.loads(meta.value.decode())
 

@@ -84,6 +84,9 @@ def test_every_struct_field_matches_the_ctypes_mirror(tmp_path):
         assert [f for _, _, f, _ in fields] == [f[0] for f in mirror._fields_], name
         for _, _, f, _ in fields:
             assert int(got[f"{name}.{f}"]) == getattr(mirror, f).offset, (name, f)
+    # the power threshold travels at the END of gpr_text_grid (power samples are snapped to it at parse time)
+    assert [f for _, _, f, _ in structs["gpr_text_grid"]][-1] == "power_threshold"
+    assert (int(got["gpr_text_grid"]), int(got["gpr_text_grid.power_threshold"])) == (48, 40)
 
 
 def test_header_is_plain_c():

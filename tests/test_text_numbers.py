@@ -4,6 +4,7 @@ path + Eisel-Lemire with the generated 128-bit table) against Python's correctly
 The parser's contract is "equal to strtod + (float), or decline" (a declined number marks the span hard and the
 CPU's strtod decides), so every ACCEPTED conversion must match bit for bit; the rate of declines on realistic input
 (17-digit DCGM_FI_PROF_GR_ENGINE_ACTIVE ratios: shortest-round-trip doubles) must be negligible."""
+import math
 import os
 import random
 import struct
@@ -130,6 +131,44 @@ def test_parse_value_declines_what_it_cannot_decide(driver):
     out = _run(driver, ["V .5", "V 5.", "V 12345678901234567890", "V 1.2.3", "V abc", "V +", "V 0x10",
                         "V 1234567890123456789012", "V 1e", "V 1e+", "V 1e1234", "V e5", "V 1.e5"])
     assert all(line.split()[0] == "0" for line in out), out
+
+
+def test_power_samples_snapped_to_the_threshold_decide_like_float64(driver):
+    """parse_value into the power plane (power_snap / snap_power): for every threshold — exact in f32 or not, tiny,
+    negative, beyond the f32 range — the stored f32 compares `>= up` (the smallest f32 >= thr, what gpr_decide
+    compares with) exactly when the float64 reading compares `>= thr`, as Prometheus does; it is the plain f32
+    rounding wherever that already agrees, and one step off it otherwise.  0 and NaN turn the snap off."""
+    import edges as E
+    rng = random.Random(150)
+    thresholds = E.THRESHOLDS + [1e-40, -5.0, 1e-3, 123456.789, 3.4028235677973366e38, 1e39]
+    cases = []
+    for thr in thresholds:
+        vals = E.power_edges(thr) + [thr * (1 + rng.uniform(-1e-7, 1e-7)) for _ in range(200)]
+        vals += [0.0, -0.0, thr / 2, thr * 2, 1e-45, 1e-50]
+        cases += [(thr, v) for v in vals if math.isfinite(v)]     # (NaN / Inf are parse_sample's, never snapped)
+    cases += [(t, 149.999999) for t in (0.0, math.nan)] + [(t, 150.5) for t in (0.0, math.nan)]
+    out = _run(driver, [f"S {thr!r} {E.go_float(v)}" for thr, v in cases])
+    f32 = lambda b: float(np.frombuffer(struct.pack("<I", b), np.float32)[0])
+    flipped = 0
+    for (thr, v), line in zip(cases, out):
+        q, bits, up, down = (int(x, 16) if i else int(x) for i, x in enumerate(line.split()))
+        assert q, (thr, v)
+        # rn: the plain f32 rounding, a non-zero value below the f32 range kept at +-denorm_min (to_f32)
+        got, rn = f32(bits), float(np.float32(v)) if np.float32(v) != 0 or v == 0 else math.copysign(f32(1), v)
+        if thr == 0 or math.isnan(thr):
+            assert got == rn, (thr, v)
+            continue
+        assert f32(up) == E.f32_up(thr) and f32(down) == float(np.nextafter(np.float32(E.f32_up(thr)), np.float32(-np.inf)))
+        assert (got >= f32(up)) == (v >= thr) and (got >= thr) == (v >= thr), (thr, v, got)
+        if (rn >= f32(up)) == (v >= thr):
+            assert got == rn, (thr, v, got, rn)
+        else:
+            flipped += 1
+            assert got in (f32(up), f32(down)), (thr, v, got)
+    # the cases that matter are there: plain rounding would have decided them wrongly
+    assert flipped >= 10
+    assert out[cases.index((150.0, 149.999999))].split()[1] == "4315ffff"        # 149.999999 -> just below 150.0f
+    assert out[cases.index((149.99, 149.99))].split()[1] == "4315fd71"           # == a decimal threshold: vetoes
 
 
 def test_parse_timestamp_is_exact_in_milliseconds(driver):
