@@ -31,9 +31,9 @@
 
 namespace {
 
-constexpr int kLdgWarps = 16;
-constexpr int kLdgUnroll = 8;
-constexpr size_t kTmaSmemBudget = 208 * 1024;
+using gpr::kLdgUnroll;
+using gpr::kLdgWarps;
+using gpr::kTmaSmemBudget;
 constexpr int kSlots = 256;      // outstanding async results
 constexpr int kMaxChunkEvents = 64;
 constexpr int kExchangeDepth = 4;  // exchange buffer sets of the fused multi-GPU path = 2 x scratch sets
@@ -280,24 +280,17 @@ float threshold_f32(double thr) { return gpr::text::threshold_up(thr); }
 
 bool power_truthy(double thr) { return thr != 0.0 && !std::isnan(thr); }
 
-gpr::TmaLayout tma_layout(const gpr_ctx* ctx, uint32_t T, int nw) {
-  gpr::TmaLayout L;
-  const uint32_t row_bytes = T * 4u;
-  const uint32_t max_chunk = (uint32_t)ctx->tma_chunk_bytes;
-  L.n_chunks = (row_bytes + max_chunk - 1) / max_chunk;
-  uint32_t ce = (T + L.n_chunks - 1) / L.n_chunks;
-  ce = (ce + 3u) & ~3u;
-  L.chunk_elems = ce;
-  L.n_chunks = (T + ce - 1) / ce;
-  L.stage_bytes = (ce * 4u + 127u) & ~127u;
-  uint32_t d = (uint32_t)((kTmaSmemBudget - 1024) / ((size_t)L.stage_bytes * nw));
-  d = std::min<uint32_t>(d, (uint32_t)ctx->tma_depth_max);
-  L.depth = std::max<uint32_t>(d, 1u);
-  return L;
-}
-
-size_t tma_smem_bytes(const gpr::TmaLayout& L, int nw) {
-  return (size_t)nw * L.depth * L.stage_bytes + (size_t)nw * L.depth * sizeof(uint64_t);
+// the context's tuning knobs as the launch geometry (gpr_launch.h) takes them
+gpr::LaunchKnobs launch_knobs(const gpr_ctx* ctx) {
+  gpr::LaunchKnobs k;
+  k.sm_count = ctx->sm_count;
+  k.variant = ctx->variant;
+  k.ldg_ctas_per_sm = ctx->ldg_ctas_per_sm;
+  k.tma_warps = ctx->tma_warps;
+  k.tma_chunk_bytes = ctx->tma_chunk_bytes;
+  k.tma_depth_max = ctx->tma_depth_max;
+  k.fold_threads = ctx->fold_threads;
+  return k;
 }
 
 // One launch helper for both variants; `pdl` adds the programmatic-stream-serialization
@@ -316,9 +309,8 @@ cudaError_t launch_ex(Kernel k, uint32_t grid, uint32_t block, size_t smem, cuda
 }
 
 template <int NW>
-cudaError_t launch_tma(gpr_ctx* ctx, const gpr::ReduceParams& rp, uint32_t grid, bool pdl) {
-  const gpr::TmaLayout L = tma_layout(ctx, rp.T, NW);
-  return launch_ex(gpr::k_reduce_tma<NW>, grid, NW * 32, tma_smem_bytes(L, NW), ctx->stream, pdl, rp, L);
+cudaError_t launch_tma(gpr_ctx* ctx, const gpr::ReduceParams& rp, const gpr::ReducePlan& plan, bool pdl) {
+  return launch_ex(gpr::k_reduce_tma<NW>, plan.grid, plan.block, plan.smem, ctx->stream, pdl, rp, plan.L);
 }
 
 // launch one reduce pass over the rows described by rp
@@ -326,30 +318,18 @@ int launch_reduce(gpr_ctx* ctx, gpr::ReduceParams& rp, bool tma_ok, bool pdl) {
   if (rp.total_rows == 0) return GPR_OK;
   // AUTO = the TMA pipeline (measured winner on H100 at C2 and C3, DESIGN.md §4.3); rows that are
   // not 16-byte aligned or have T % 4 != 0 cannot be bulk-copied and take the LDG kernel
-  int variant = ctx->variant == GPR_KERNEL_AUTO ? GPR_KERNEL_TMA : ctx->variant;
-  if (variant == GPR_KERNEL_TMA && !tma_ok) variant = GPR_KERNEL_LDG;
-  if (variant == GPR_KERNEL_TMA &&
-      tma_smem_bytes(tma_layout(ctx, rp.T, ctx->tma_warps), ctx->tma_warps) > kTmaSmemBudget)
-    variant = GPR_KERNEL_LDG;  // a tuning override (GPR_TMA_WARPS / GPR_TMA_CHUNK) that does not fit
+  const gpr::ReducePlan plan = gpr::plan_reduce(launch_knobs(ctx), rp.T, rp.total_rows, tma_ok, rp.util_u8 != 0);
   cudaError_t e;
-  if (rp.util_u8) {  // biased-byte util plane: one kernel, any alignment (the power plane stays f32)
-    uint32_t grid = (uint32_t)(ctx->sm_count * ctx->ldg_ctas_per_sm);
-    const uint32_t need = (rp.total_rows + kLdgWarps - 1) / kLdgWarps;
-    grid = std::max<uint32_t>(1u, std::min<uint32_t>(grid, need));
-    e = launch_ex(gpr::k_reduce_u8<kLdgWarps, 4>, grid, kLdgWarps * 32, 0, ctx->stream, pdl, rp);
-  } else if (variant == GPR_KERNEL_TMA) {
+  if (plan.kernel == gpr::kReduceU8) {
+    e = launch_ex(gpr::k_reduce_u8<kLdgWarps, gpr::kU8Unroll>, plan.grid, plan.block, 0, ctx->stream, pdl, rp);
+  } else if (plan.kernel == gpr::kReduceTma) {
     const int nw = ctx->tma_warps;
-    uint32_t grid = (uint32_t)ctx->sm_count;
-    grid = std::max<uint32_t>(1u, std::min<uint32_t>(grid, (rp.total_rows + nw - 1) / nw));
-    if (nw == 4) e = launch_tma<4>(ctx, rp, grid, pdl);
-    else if (nw == 16) e = launch_tma<16>(ctx, rp, grid, pdl);
-    else if (nw == 32) e = launch_tma<32>(ctx, rp, grid, pdl);
-    else e = launch_tma<8>(ctx, rp, grid, pdl);
+    if (nw == 4) e = launch_tma<4>(ctx, rp, plan, pdl);
+    else if (nw == 16) e = launch_tma<16>(ctx, rp, plan, pdl);
+    else if (nw == 32) e = launch_tma<32>(ctx, rp, plan, pdl);
+    else e = launch_tma<8>(ctx, rp, plan, pdl);
   } else {
-    uint32_t grid = (uint32_t)(ctx->sm_count * ctx->ldg_ctas_per_sm);
-    const uint32_t need = (rp.total_rows + kLdgWarps - 1) / kLdgWarps;
-    grid = std::max<uint32_t>(1u, std::min<uint32_t>(grid, need));
-    e = launch_ex(gpr::k_reduce_ldg<kLdgWarps, kLdgUnroll>, grid, kLdgWarps * 32, 0, ctx->stream, pdl, rp);
+    e = launch_ex(gpr::k_reduce_ldg<kLdgWarps, kLdgUnroll>, plan.grid, plan.block, 0, ctx->stream, pdl, rp);
   }
   ctx->launches++;
   CU(e);
@@ -578,8 +558,8 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
   // the fold grid: 32 bitmap words per CTA and round; a handful of CTAs even at millions of pods
   // one bitmap word per warp and round, 4 words per warp in flight (fold_words<4>): small CTAs spread the fold's
   // loads over many SMs — each SM's path to L2 is busy with the next decision's reduce CTA
-  const uint32_t fold_threads = (uint32_t)ctx->fold_threads, fold_warps = fold_threads / 32u;
-  const uint32_t fold_grid = std::max<uint32_t>(1u, std::min<uint32_t>((W + 4u * fold_warps - 1u) / (4u * fold_warps), (uint32_t)ctx->sm_count));
+  const uint32_t fold_threads = (uint32_t)ctx->fold_threads;
+  const uint32_t fold_grid = gpr::fold_grid(launch_knobs(ctx), P);
 
   if (!async) {
     CU(cudaEventRecord(ctx->ev_k0, ctx->stream));

@@ -29,6 +29,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "gpr_launch.h"
+
 namespace gpr {
 
 // ------------------------------------------------------------------------------------------
@@ -552,9 +554,12 @@ __device__ __forceinline__ const float* row_ptr(const ReduceParams& p, uint32_t 
   return base + (size_t)local * p.ld;
 }
 
-// rows owned by this CTA under the strided assignment row = blockIdx.x + j * gridDim.x
+// rows owned by this CTA under the strided assignment row = blockIdx.x + j * gridDim.x.  In 64 bits: with a power
+// plane total_rows reaches 2^32 - 2, and adding gridDim.x - 1 to it would wrap.
 __device__ __forceinline__ uint32_t cta_row_count(uint32_t total_rows) {
-  return total_rows > blockIdx.x ? (total_rows - blockIdx.x + gridDim.x - 1) / gridDim.x : 0u;
+  return total_rows > blockIdx.x
+             ? (uint32_t)(((uint64_t)total_rows - blockIdx.x + gridDim.x - 1) / gridDim.x)
+             : 0u;
 }
 
 // before a warp's first publish: the decision that last used this scratch set must have folded
@@ -782,12 +787,18 @@ __device__ __forceinline__ uint64_t l2_evict_first_policy() {
   return pol;
 }
 
+// The ring layout, chosen on the host by gpr_launch.h's tma_layout.  The same definition is in gpr_launch.h; the guard
+// keeps whichever comes first, so that this header's namespace body also stands alone (the CPU emulation of the
+// kernels compiles it without the host header).
+#ifndef GPR_TMA_LAYOUT_DEFINED
+#define GPR_TMA_LAYOUT_DEFINED
 struct TmaLayout {
   uint32_t depth;         // stages per warp
   uint32_t stage_bytes;   // capacity of one stage (multiple of 128)
   uint32_t chunk_elems;   // elements copied per chunk (multiple of 4); a row = n_chunks chunks
   uint32_t n_chunks;
 };
+#endif
 
 // Requirements (checked on the host): every row base 16-byte aligned, T % 4 == 0.
 //
@@ -811,7 +822,7 @@ __global__ void __launch_bounds__(NW * 32) k_reduce_tma(ReduceParams p, TmaLayou
 
   pdl_launch_dependents();
   const uint32_t n_rows = cta_row_count(p.total_rows);
-  const uint32_t my_rows = n_rows > w ? (n_rows - w + NW - 1) / NW : 0u;
+  const uint32_t my_rows = n_rows > w ? (uint32_t)(((uint64_t)n_rows - w + NW - 1) / NW) : 0u;  // (grid 1: n_rows ~ 2^32)
   bool scratch_ok = false;
   const uint32_t n_items = my_rows * L.n_chunks;
 

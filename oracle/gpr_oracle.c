@@ -123,7 +123,7 @@ typedef struct {
   uint32_t p0, p1, G, T;
   uint64_t ld;
   double thr;
-  uint32_t *dbits, *cbits;
+  uint32_t *dbits, *cbits, *vbits;
   float *smax;
   uint64_t counts[3];
   /* synthetic streaming mode */
@@ -409,12 +409,15 @@ static void *synth_job(void *arg) {
     for (uint32_t g = 0; g < G; ++g) {
       const uint64_t s = (j->pod_offset + p) * G + g;
       fill_row(j->seed, 0, s, T, urow);
-      if (gpo_max_over_time(urow, T) == 0.0) ++idle_series;
+      const double m = gpo_max_over_time(urow, T);
+      if (j->smax) j->smax[(uint64_t)p * G + g] = (float)m;
+      if (m == 0.0) ++idle_series;
       if (use_power) {
         fill_row(j->seed, 1, s, T, wrow);
         if (gpo_max_over_time(wrow, T) >= j->thr) veto = 1;
       }
     }
+    if (veto && j->vbits) j->vbits[p >> 5] |= 1u << (p & 31);
     const int candidate = idle_series > 0 && !veto;
     const int elig = j->use_elig ? gpo_synth_eligible_pod(j->seed, j->pod_offset + p) : 1;
     if (candidate) {
@@ -435,14 +438,22 @@ static void *synth_job(void *arg) {
 int gpo_decide_synth(int n_threads, uint64_t seed, uint64_t pod_offset, uint32_t P, uint32_t G,
                      uint32_t T, int use_power, double thr, int use_elig, uint32_t *dbits,
                      uint32_t *cbits, uint64_t counts[3]) {
+  return gpo_decide_synth_ex(n_threads, seed, pod_offset, P, G, T, use_power, thr, use_elig, dbits, cbits, NULL,
+                             NULL, counts);
+}
+
+int gpo_decide_synth_ex(int n_threads, uint64_t seed, uint64_t pod_offset, uint32_t P, uint32_t G,
+                        uint32_t T, int use_power, double thr, int use_elig, uint32_t *dbits,
+                        uint32_t *cbits, float *smax, uint32_t *vbits, uint64_t counts[3]) {
   if (n_threads < 1) n_threads = 1;
   zero_bits(dbits, P);
   zero_bits(cbits, P);
+  zero_bits(vbits, P);
   job_t *jobs = (job_t *)calloc((size_t)n_threads, sizeof(job_t));
   if (!jobs) return -1;
   for (int i = 0; i < n_threads; ++i) {
     job_t *j = &jobs[i];
-    j->G = G, j->T = T, j->thr = thr, j->dbits = dbits, j->cbits = cbits;
+    j->G = G, j->T = T, j->thr = thr, j->dbits = dbits, j->cbits = cbits, j->smax = smax, j->vbits = vbits;
     j->seed = seed, j->pod_offset = pod_offset, j->use_power = use_power, j->use_elig = use_elig;
     j->p0 = split32(P, n_threads, i);
     j->p1 = split32(P, n_threads, i + 1);

@@ -59,6 +59,13 @@ int gpo_decide_synth(int n_threads, uint64_t seed, uint64_t pod_offset, uint32_t
                      uint32_t n_gpus, uint32_t n_samples, int use_power, double power_threshold,
                      int use_elig, uint32_t *decision_bits, uint32_t *candidate_bits,
                      uint64_t counts[3]);
+/* Same, plus the window max of every util series (series_max[p * n_gpus + g], may be NULL) and the pods the
+ * power clause vetoes (veto_bits, may be NULL): together they check every row of a window, also rows that
+ * change no verdict bit.                                                                    */
+int gpo_decide_synth_ex(int n_threads, uint64_t seed, uint64_t pod_offset, uint32_t n_pods,
+                        uint32_t n_gpus, uint32_t n_samples, int use_power, double power_threshold,
+                        int use_elig, uint32_t *decision_bits, uint32_t *candidate_bits,
+                        float *series_max, uint32_t *veto_bits, uint64_t counts[3]);
 
 /* CPUs this process may run on (affinity-mask aware) */
 int gpo_hardware_threads(void);

@@ -48,6 +48,9 @@ def load() -> C.CDLL:
         lib.gpo_decide_synth.restype = C.c_int
         lib.gpo_decide_synth.argtypes = [C.c_int, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint32,
                                          C.c_uint32, C.c_int, C.c_double, C.c_int, _P, _P, _P]
+        lib.gpo_decide_synth_ex.restype = C.c_int
+        lib.gpo_decide_synth_ex.argtypes = [C.c_int, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint32,
+                                            C.c_uint32, C.c_int, C.c_double, C.c_int, _P, _P, _P, _P, _P]
         lib.gpo_hardware_threads.restype = C.c_int
         lib.gpo_pool_pin.restype = None
         lib.gpo_pool_pin.argtypes = [C.c_int]
@@ -109,21 +112,30 @@ def synth_eligible(seed, pod_offset, P):
 
 
 def decide_synth(seed, pod_offset, P, G, T, use_power=False, power_threshold=0.0, use_elig=False,
-                 n_threads: int = 0):
+                 n_threads: int = 0, want_series_max: bool = False, want_veto: bool = False):
+    """want_series_max: also the window max of every util series ([P, G] float32); want_veto: also the packed
+    bitmap of the pods the power clause vetoes"""
     if n_threads <= 0:
         n_threads = hardware_threads()
     W = max((P + 31) // 32, 1)
     dbits = np.zeros(W, dtype=np.uint32)
     cbits = np.zeros(W, dtype=np.uint32)
+    vbits = np.zeros(W, dtype=np.uint32) if want_veto else None
+    smax = np.empty((P, G), dtype=np.float32) if want_series_max else None
     counts = np.zeros(3, dtype=np.uint64)
-    rc = load().gpo_decide_synth(n_threads, seed, pod_offset, P, G, T, int(use_power),
-                                 float(power_threshold), int(use_elig), _p(dbits), _p(cbits),
-                                 _p(counts))
+    rc = load().gpo_decide_synth_ex(n_threads, seed, pod_offset, P, G, T, int(use_power),
+                                    float(power_threshold), int(use_elig), _p(dbits), _p(cbits),
+                                    _p(smax), _p(vbits), _p(counts))
     if rc != 0:
         raise RuntimeError("gpo_decide_synth failed")
     W = (P + 31) // 32
-    return {"decision_bits": dbits[:W], "candidate_bits": cbits[:W], "n_series": int(counts[0]),
-            "n_candidates": int(counts[1]), "n_decisions": int(counts[2])}
+    out = {"decision_bits": dbits[:W], "candidate_bits": cbits[:W], "n_series": int(counts[0]),
+           "n_candidates": int(counts[1]), "n_decisions": int(counts[2])}
+    if want_series_max:
+        out["series_max"] = smax
+    if want_veto:
+        out["veto_bits"] = vbits[:W]
+    return out
 
 
 def pool_pin(on: bool = True):

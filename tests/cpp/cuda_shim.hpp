@@ -183,17 +183,26 @@ static inline unsigned int atomicCAS(unsigned int* p, unsigned int expect, unsig
 }
 
 // ---- launching a grid ------------------------------------------------------------------------------------------
+// CTAs resident at once (0 = the whole grid).  A kernel whose CTAs never wait for one another — the reduce kernels,
+// the single-GPU fold — may run in waves, as on a device with fewer SMs than CTAs; a wide grid of 1024-thread CTAs
+// then does not need thousands of threads at once.
+static unsigned g_max_resident_ctas = 0;
+
 template <class Fn>
 static void launch(unsigned grid, unsigned threads, size_t smem, Fn&& kernel) {
-  std::vector<std::unique_ptr<CtaCtx>> ctas;
-  std::vector<std::thread> th;
-  for (unsigned c = 0; c < grid; ++c) ctas.push_back(std::make_unique<CtaCtx>(threads, smem));
-  for (unsigned c = 0; c < grid; ++c)
-    for (unsigned t = 0; t < threads; ++t)
-      th.emplace_back([&, c, t] {
-        threadIdx.x = t, blockIdx.x = c, blockDim.x = threads, gridDim.x = grid;
-        tl_cta = ctas[c].get();
-        kernel();
-      });
-  for (auto& t : th) t.join();
+  const unsigned wave = g_max_resident_ctas ? g_max_resident_ctas : std::max(grid, 1u);
+  for (unsigned c0 = 0; c0 < grid; c0 += wave) {
+    const unsigned c1 = std::min(grid, c0 + wave);
+    std::vector<std::unique_ptr<CtaCtx>> ctas;
+    std::vector<std::thread> th;
+    for (unsigned c = c0; c < c1; ++c) ctas.push_back(std::make_unique<CtaCtx>(threads, smem));
+    for (unsigned c = c0; c < c1; ++c)
+      for (unsigned t = 0; t < threads; ++t)
+        th.emplace_back([&, c, t] {
+          threadIdx.x = t, blockIdx.x = c, blockDim.x = threads, gridDim.x = grid;
+          tl_cta = ctas[c - c0].get();
+          kernel();
+        });
+    for (auto& t : th) t.join();
+  }
 }

@@ -63,3 +63,20 @@ def test_streaming_decision_equals_materialised(oracle_c):
     d = oracle_c.decide_synth(SEED, 64, P, G, T)
     assert np.array_equal(c["decision_bits"], d["decision_bits"])
     assert 0 < c["n_decisions"] < P
+
+
+def test_streaming_decision_series_max_and_veto(oracle_c, oracle_np):
+    """decide_synth's optional outputs (used to check every row of device windows too large for host RAM)"""
+    import kat
+    P, G, T = 203, 3, 61
+    b = oracle_c.decide_synth(SEED, 5, P, G, T, use_power=True, power_threshold=150.0, use_elig=True, n_threads=3,
+                              want_series_max=True, want_veto=True)
+    u = oracle_c.synth_fill(SEED, 0, 5, P, G, T)
+    w = oracle_c.synth_fill(SEED, 1, 5, P, G, T)
+    a = oracle_np.decide(u, w, oracle_c.synth_eligible(SEED, 5, P), None, 0, 150.0)
+    for k in ("decision_bits", "candidate_bits", "veto_bits", "n_series", "n_candidates", "n_decisions"):
+        assert np.array_equal(a[k], b[k]), k
+    assert kat.smax_equal(b["series_max"], a["series_max"])
+    assert 0 < int(np.unpackbits(b["veto_bits"].view(np.uint8)).sum()) < P
+    c = oracle_c.decide_synth(SEED, 5, P, G, T, want_veto=True)      # no power clause: nobody is vetoed
+    assert not c["veto_bits"].any()
