@@ -26,6 +26,7 @@
 #include <vector>
 
 #include "gpr_kernels.cuh"
+#include "gpr_ring.cuh"
 #include "gpr_synth.cuh"
 #include "gpr_text_kernels.cuh"
 
@@ -160,6 +161,9 @@ struct gpr_ctx {
   float* d_idx_util = nullptr;
   float* d_idx_power = nullptr;
   uint32_t idx_ld = 0;      // padded to a multiple of 4 (TMA-able rows), padding stays NaN
+  // gpr_text_parse(GPR_TEXT_RESIDENT) merged samples into the ring behind the index's back: deciding on the index
+  // is refused until gpr_resident_reindex has rebuilt it
+  bool idx_stale = false;
   float* d_cols = nullptr;
   size_t cols_cap = 0;
 
@@ -377,6 +381,9 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
     util = ctx->d_res_util;
     power = ctx->d_res_power;
     if (ctx->d_idx_util) {  // decide on the block-maxima index: same verdict, T/64 of the bytes
+      if (ctx->idx_stale)
+        return fail(ctx, GPR_E_STATE, "the block index is stale: gpr_text_parse(GPR_TEXT_RESIDENT) merged samples "
+                    "into the ring; call gpr_resident_reindex before gpr_decide_resident");
       T = ctx->idx_ld, ld = ctx->idx_ld;
       util = ctx->d_idx_util;
       power = ctx->d_idx_power;
@@ -704,65 +711,6 @@ int sync_impl(gpr_ctx* ctx) {
                 "the results of this batch are not global", gpr::kPeerTimeoutNs / 1000000000ull);
   }
   return GPR_OK;
-}
-
-constexpr uint32_t kIdxBlock = 64;
-
-// NaN-skipping max of block b (samples [64 b, 64 b + 64) of one resident row), one warp
-__device__ __forceinline__ float block_max_warp(const float* row, uint32_t T, uint32_t b, int lane) {
-  const uint32_t t0 = b * kIdxBlock;
-  float m = gpr::nan_f();
-  for (uint32_t t = t0 + lane; t < min(T, t0 + kIdxBlock); t += 32) m = fmaxf(m, row[t]);
-  return gpr::warp_max(m);
-}
-
-// Scatter n_new columns of every row into the time ring; with an index, recompute the maxima of the
-// blocks the new columns landed in (the overwritten samples may have been the old maximum).
-__global__ void __launch_bounds__(128) k_append(float* __restrict__ dst, const float* __restrict__ src,
-                                               uint32_t n_rows, uint32_t T, uint32_t head, uint32_t n_new,
-                                               uint64_t ld_src, float* __restrict__ idx, uint32_t idx_ld) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
-  for (uint32_t r = blockIdx.x; r < n_rows; r += gridDim.x) {
-    float* out = dst + (size_t)r * T;
-    const float* in = src + (size_t)r * ld_src;
-    for (uint32_t j = threadIdx.x; j < n_new; j += blockDim.x) {
-      uint32_t t = head + j;
-      if (t >= T) t -= T;
-      out[t] = in[j];
-    }
-    if (idx) {
-      __syncthreads();  // this CTA's column stores are visible to its own warps
-      // touched blocks: those of [head, head + n_new) modulo T — at most two contiguous runs
-      const uint32_t n_blocks = (T + kIdxBlock - 1) / kIdxBlock;
-      const uint32_t first = head / kIdxBlock;
-      const uint32_t span_end = head + n_new;  // exclusive, may exceed T (wraps)
-      const uint32_t last = (min(span_end, T) - 1) / kIdxBlock;
-      for (uint32_t b = first + warp; b <= last; b += n_warps) {
-        const float m = block_max_warp(out, T, b, lane);
-        if (lane == 0) idx[(size_t)r * idx_ld + b] = m;
-      }
-      if (span_end > T) {  // wrapped part [0, span_end - T)
-        const uint32_t wlast = min((span_end - T - 1) / kIdxBlock, n_blocks - 1);
-        for (uint32_t b = warp; b <= wlast; b += n_warps) {
-          const float m = block_max_warp(out, T, b, lane);
-          if (lane == 0) idx[(size_t)r * idx_ld + b] = m;
-        }
-      }
-      __syncthreads();
-    }
-  }
-}
-
-// full rebuild of the index (after the caller wrote the resident planes directly)
-__global__ void __launch_bounds__(128) k_reindex(const float* __restrict__ plane, uint32_t n_rows, uint32_t T,
-                                                float* __restrict__ idx, uint32_t idx_ld) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
-  const uint32_t n_blocks = (T + kIdxBlock - 1) / kIdxBlock;
-  for (uint32_t r = blockIdx.x; r < n_rows; r += gridDim.x)
-    for (uint32_t b = warp; b < n_blocks; b += n_warps) {
-      const float m = block_max_warp(plane + (size_t)r * T, T, b, lane);
-      if (lane == 0) idx[(size_t)r * idx_ld + b] = m;
-    }
 }
 
 }  // namespace
@@ -1167,7 +1115,7 @@ int gpr_resident_init(gpr_ctx* ctx, uint32_t P, uint32_t G, uint32_t T, uint32_t
   if (ctx->d_idx_power) CU(cudaFree(ctx->d_idx_power));
   ctx->d_idx_util = ctx->d_idx_power = nullptr, ctx->idx_ld = 0;
   if (flags & GPR_F_BLOCK_INDEX) {
-    ctx->idx_ld = (((T + kIdxBlock - 1) / kIdxBlock) + 3u) & ~3u;
+    ctx->idx_ld = gpr::index_ld(T);
     const size_t ib = (size_t)P * G * ctx->idx_ld * sizeof(float);
     CU(cudaMalloc(reinterpret_cast<void**>(&ctx->d_idx_util), ib));
     CU(cudaMemsetAsync(ctx->d_idx_util, 0xFF, ib, ctx->stream));
@@ -1178,6 +1126,7 @@ int gpr_resident_init(gpr_ctx* ctx, uint32_t P, uint32_t G, uint32_t T, uint32_t
   }
   CU(cudaStreamSynchronize(ctx->stream));
   ctx->res_P = P, ctx->res_G = G, ctx->res_T = T, ctx->res_head = 0;
+  ctx->idx_stale = false;
   return GPR_OK;
   GPR_CATCH(ctx)
 }
@@ -1190,15 +1139,16 @@ int gpr_resident_reindex(gpr_ctx* ctx) {
   CU(cudaSetDevice(ctx->device));
   ctx->last_was_reduce = false;
   const size_t rows = (size_t)ctx->res_P * ctx->res_G;
-  const uint32_t grid = (uint32_t)std::min<size_t>(rows, (size_t)ctx->sm_count * 16);
-  k_reindex<<<grid, 128, 0, ctx->stream>>>(ctx->d_res_util, (uint32_t)rows, ctx->res_T, ctx->d_idx_util,
-                                           ctx->idx_ld);
+  const uint32_t grid = gpr::ring_grid(rows, ctx->sm_count);
+  gpr::k_reindex<<<grid, gpr::kRingThreads, 0, ctx->stream>>>(ctx->d_res_util, (uint32_t)rows, ctx->res_T,
+                                                             ctx->d_idx_util, ctx->idx_ld);
   if (ctx->d_res_power)
-    k_reindex<<<grid, 128, 0, ctx->stream>>>(ctx->d_res_power, (uint32_t)rows, ctx->res_T, ctx->d_idx_power,
-                                             ctx->idx_ld);
+    gpr::k_reindex<<<grid, gpr::kRingThreads, 0, ctx->stream>>>(ctx->d_res_power, (uint32_t)rows, ctx->res_T,
+                                                               ctx->d_idx_power, ctx->idx_ld);
   ctx->launches += ctx->d_res_power ? 2 : 1;
   CU(cudaGetLastError());
   CU(cudaStreamSynchronize(ctx->stream));
+  ctx->idx_stale = false;
   return GPR_OK;
   GPR_CATCH(ctx)
 }
@@ -1219,14 +1169,23 @@ int gpr_append(gpr_ctx* ctx, const float* util_cols, const float* power_cols, ui
   uint64_t ld = row_stride ? row_stride : n_new;
   if (ld < n_new) return fail(ctx, GPR_E_INVALID, "row_stride < n_new");
   // only the newest T columns can survive in a ring of T
-  uint32_t skip = n_new > T ? n_new - T : 0;
-  const uint32_t n_eff = n_new - skip;
-  const float* planes_in[2] = {util_cols, ctx->d_res_power ? power_cols : nullptr};
+  const gpr::RingSpan sp = gpr::ring_span(ctx->res_head, n_new, T);
+  const uint32_t n_eff = sp.n;
+  const uint32_t grid = gpr::ring_grid(rows, ctx->sm_count);
+  const float* planes_in[2] = {util_cols, power_cols};
   float* planes_out[2] = {ctx->d_res_util, ctx->d_res_power};
   float* planes_idx[2] = {ctx->d_idx_util, ctx->d_idx_power};
   for (int pl = 0; pl < 2; ++pl) {
-    if (!planes_in[pl]) continue;
-    const float* src = planes_in[pl] + skip;
+    const gpr::RingLaunch what = gpr::append_launch(planes_out[pl] != nullptr, planes_in[pl] != nullptr);
+    if (what == gpr::kRingNone) continue;
+    if (what == gpr::kRingOpen) {  // no columns for this plane: its new buckets hold no sample
+      gpr::k_open<<<grid, gpr::kRingThreads, 0, ctx->stream>>>(planes_out[pl], (uint32_t)rows, T, sp.start, sp.n,
+                                                               planes_idx[pl], ctx->idx_ld);
+      ctx->launches++;
+      CU(cudaGetLastError());
+      continue;
+    }
+    const float* src = planes_in[pl] + sp.src_col;
     uint64_t ld_dev = ld;
     if (mem_kind == GPR_MEM_HOST) {
       int rc = grow(ctx, &ctx->d_cols, &ctx->cols_cap, rows * n_eff + 4);
@@ -1240,14 +1199,12 @@ int gpr_append(gpr_ctx* ctx, const float* util_cols, const float* power_cols, ui
       src = ctx->d_cols;
       ld_dev = n_eff;
     }
-    const uint32_t grid = (uint32_t)std::min<size_t>(rows, (size_t)ctx->sm_count * 16);
-    k_append<<<grid, 128, 0, ctx->stream>>>(planes_out[pl], src, (uint32_t)rows, T,
-                                            (ctx->res_head + skip) % T, n_eff, ld_dev, planes_idx[pl],
-                                            ctx->idx_ld);
+    gpr::k_append<<<grid, gpr::kRingThreads, 0, ctx->stream>>>(planes_out[pl], src, (uint32_t)rows, T, sp.start,
+                                                               sp.n, ld_dev, planes_idx[pl], ctx->idx_ld);
     ctx->launches++;
     CU(cudaGetLastError());
   }
-  ctx->res_head = (uint32_t)(((uint64_t)ctx->res_head + n_new) % T);
+  ctx->res_head = sp.next_head;
   CU(cudaStreamSynchronize(ctx->stream));
   return GPR_OK;
   GPR_CATCH(ctx)
@@ -1278,10 +1235,19 @@ int gpr_resident_advance(gpr_ctx* ctx, uint32_t n_new) {
   ctx->last_was_reduce = false;
   const uint32_t T = ctx->res_T;
   const size_t rows = (size_t)ctx->res_P * ctx->res_G;
+  const gpr::RingSpan sp = gpr::ring_span(ctx->res_head, n_new, T);
   float* planes[2] = {ctx->d_res_util, ctx->d_res_power};
-  for (float* pl : planes) {
-    if (!pl) continue;
-    if (n_new >= T) {
+  float* planes_idx[2] = {ctx->d_idx_util, ctx->d_idx_power};
+  for (int k = 0; k < 2; ++k) {
+    float* pl = planes[k];
+    const gpr::RingLaunch what = gpr::advance_launch(pl != nullptr, planes_idx[k] != nullptr);
+    if (what == gpr::kRingNone) continue;
+    if (what == gpr::kRingOpen) {  // the opened buckets' old samples leave the index too
+      gpr::k_open<<<gpr::ring_grid(rows, ctx->sm_count), gpr::kRingThreads, 0, ctx->stream>>>(
+          pl, (uint32_t)rows, T, sp.start, sp.n, planes_idx[k], ctx->idx_ld);
+      ctx->launches++;
+      CU(cudaGetLastError());
+    } else if (n_new >= T) {
       CU(cudaMemsetAsync(pl, 0xFF, rows * (size_t)T * sizeof(float), ctx->stream));
     } else {
       const uint64_t total = (uint64_t)rows * n_new;
@@ -1291,7 +1257,7 @@ int gpr_resident_advance(gpr_ctx* ctx, uint32_t n_new) {
       CU(cudaGetLastError());
     }
   }
-  ctx->res_head = (uint32_t)(((uint64_t)ctx->res_head + n_new) % T);
+  ctx->res_head = sp.next_head;
   CU(cudaStreamSynchronize(ctx->stream));
   return GPR_OK;
   GPR_CATCH(ctx)
@@ -1722,6 +1688,7 @@ int gpr_text_parse(gpr_ctx* ctx, int32_t slot, gpr_text_span* spans, uint32_t n_
     if (!pl) return fail(ctx, GPR_E_STATE, "the resident window has no power plane");
     g.ld = ctx->res_T;
     g.col_end = (ctx->res_head + ctx->res_T - 1) % ctx->res_T;  // the newest bucket sits just before the head
+    if (ctx->d_idx_util) ctx->idx_stale = true;  // the merge does not touch the index (gpr_resident_reindex)
   } else {
     const size_t cells = (size_t)n_rows * n_samples;
     const size_t cap_before = ctx->tplane_cap[plane];

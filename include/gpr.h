@@ -91,8 +91,10 @@ enum {
 /* ---- gpr_config.flags ---------------------------------------------------------------- */
 #define GPR_F_POWER_PLANE 0x1u /* reserve staging for the power plane (host windows)      */
 #define GPR_F_BLOCK_INDEX 0x2u /* gpr_resident_init: keep the max of every 64-sample block of the
-                                  resident rows up to date in gpr_append and decide on that index —
-                                  identical verdict and series_max, 1/64 of the bytes per tick      */
+                                  resident rows up to date in gpr_append / gpr_resident_advance and
+                                  decide on that index — identical verdict and series_max, 1/64 of
+                                  the bytes per tick.  After gpr_text_parse(GPR_TEXT_RESIDENT) or
+                                  direct writes call gpr_resident_reindex (see there)              */
 
 typedef struct gpr_ctx gpr_ctx;
 
@@ -217,17 +219,23 @@ GPR_API int gpr_decide_batch_async(gpr_ctx *ctx, const gpr_window *windows, gpr_
  * irrelevant to the verdict.                                                              */
 GPR_API int gpr_resident_init(gpr_ctx *ctx, uint32_t n_pods, uint32_t n_gpus, uint32_t n_samples,
                       uint32_t flags /* GPR_F_POWER_PLANE | GPR_F_BLOCK_INDEX */);
-/* new columns laid out [p][g][n_new] (row_stride 0 = n_new); power_cols may be NULL (its
- * cells stored by the power rule of gpr_window.power_threshold).                          */
+/* new columns laid out [p][g][n_new] (row_stride 0 = n_new); power cells stored by the power
+ * rule of gpr_window.power_threshold.  power_cols may be NULL: the power plane (if any) then
+ * has no sample in the new buckets, as after gpr_resident_advance.  Only the newest n_samples
+ * of the columns are kept.  With GPR_F_BLOCK_INDEX the index blocks of the new buckets are
+ * recomputed.                                                                             */
 GPR_API int gpr_append(gpr_ctx *ctx, const float *util_cols, const float *power_cols, uint32_t n_new,
                uint64_t row_stride, int32_t mem_kind);
 /* Open the next n_new buckets of the ring without data: their columns become "no sample" in every row of
- * every resident plane and the ring head moves on.  The tick's samples are then merged in by
- * gpr_text_parse(GPR_TEXT_RESIDENT) (device-side ingest of the tick's range-query slice).  With
- * GPR_F_BLOCK_INDEX call gpr_resident_reindex after the parse.                                      */
+ * every resident plane and the ring head moves on; with GPR_F_BLOCK_INDEX their index blocks are recomputed.
+ * The tick's samples are then merged in by gpr_text_parse(GPR_TEXT_RESIDENT) (device-side ingest of the
+ * tick's range-query slice), which leaves the index stale: call gpr_resident_reindex after the parse,
+ * before gpr_decide_resident (which returns GPR_E_STATE on a stale index).                          */
 GPR_API int gpr_resident_advance(gpr_ctx *ctx, uint32_t n_new);
-/* rebuild the GPR_F_BLOCK_INDEX index after writing the resident planes directly
- * (gpr_resident_planes); a no-op without an index                                          */
+/* rebuild the GPR_F_BLOCK_INDEX index from the resident planes; a no-op without an index.  Required
+ * after gpr_text_parse(GPR_TEXT_RESIDENT) (the library marks the index stale and refuses to decide on
+ * it) and after writing the planes directly through gpr_resident_planes (which the library cannot
+ * see: deciding before the rebuild gives the verdict of the old index, without an error).          */
 GPR_API int gpr_resident_reindex(gpr_ctx *ctx);
 /* win->util / win->power are ignored (resident planes are used); gates come from win.     */
 GPR_API int gpr_decide_resident(gpr_ctx *ctx, const gpr_window *win, gpr_result *res);
