@@ -499,6 +499,8 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
     dbits_dev = my_gather + (size_t)ctx->rank * ctx->p2p_stride;   // this rank's slot: [decision | candidate]
     cbits_dev = dbits_dev + W;
   }
+  // (a series_max target also tells the reduce kernels to read every row whole: the true max is an output; without
+  // one they stop reading a row at the first sample that settles its flag, gpr_kernels.cuh "early exit")
   float* smax_dev = want_smax ? (host_out ? ctx->d_smax : res->series_max) : nullptr;
 
   gpr::FoldParams fp;

@@ -581,14 +581,33 @@ __device__ __forceinline__ void publish_row(const ReduceParams& p, uint32_t seg,
 }
 
 // ------------------------------------------------------------------------------------------
+// early exit
+// ------------------------------------------------------------------------------------------
+// The verdict needs two yes/no answers, not the max: util `max == 0`, power `max >= thr`.  A max
+// over part of a row settles its flag once it is > 0 (util: not idle, whatever follows) or >= thr
+// (power: vetoed); NaN, zeros and negatives settle nothing, a denormal positive does (no ftz, K7).
+// A row may stop being read at the first read sample that settles it, unless the call asks for
+// series_max: the true max is an output then, and every row is read in full.  An idle row — the
+// only kind n_series counts — is always read to its end, so every output is what a full read gives.
+__device__ __forceinline__ bool settles(float m, bool is_power, float thr) {
+  return is_power ? m >= thr : m > 0.0f;
+}
+__device__ __forceinline__ bool rows_may_stop(const ReduceParams& p) {
+  return p.seg[0].smax == nullptr && p.seg[1].smax == nullptr;
+}
+
+// ------------------------------------------------------------------------------------------
 // reduce, variant 1: vectorised streaming loads
 // ------------------------------------------------------------------------------------------
 // One warp per series row; rows of a CTA's contiguous range are handed out through a
 // shared-memory counter so the SM stays busy until its range is exhausted.  Any base
-// alignment / T / stride is accepted: a scalar head peels to 16-byte alignment, the body is
-// float4, a scalar tail finishes the row.
+// alignment / T / stride is accepted: a scalar peel to 16-byte alignment, a float4 body, a
+// scalar tail.  With `stop`, the peel plus the body's first 16-byte load per lane is the row's
+// head; after it and after every batch of U loads the warp leaves once a lane has seen a
+// sample that settles the row (nothing is loaded ahead of that test).
 template <int U>
-__device__ __forceinline__ float row_max_ldg(const float* __restrict__ row, uint32_t T, int lane) {
+__device__ __forceinline__ float row_max_ldg(const float* __restrict__ row, uint32_t T, int lane, bool stop,
+                                             bool is_power, float thr) {
   float m = nan_f();
   const uintptr_t a = reinterpret_cast<uintptr_t>(row);
   uint32_t head = (uint32_t)(((16u - (a & 15u)) & 15u) >> 2);
@@ -596,26 +615,33 @@ __device__ __forceinline__ float row_max_ldg(const float* __restrict__ row, uint
   if ((uint32_t)lane < head) m = __ldg(row + lane);
   const float4* __restrict__ v = reinterpret_cast<const float4*>(row + head);
   const uint32_t nv = (T - head) >> 2;
-  uint32_t i = lane;
+  uint32_t b = 0;  // first float4 of the warp's next batch (warp-uniform: the tests below are warp-wide)
+  if (stop) {
+    if ((uint32_t)lane < nv) m = fold4(m, ldg_stream(v + lane));
+    b = 32u;
+    if (__ballot_sync(0xffffffffu, settles(m, is_power, thr))) return warp_max(m);
+  }
   // full batches: U independent 16-byte loads per lane in flight
-  for (; i + 32u * (U - 1) < nv; i += 32u * U) {
+  for (; b + 32u * U <= nv; b += 32u * U) {
     float4 x[U];
 #pragma unroll
-    for (int j = 0; j < U; ++j) x[j] = ldg_stream(v + i + 32u * j);
+    for (int j = 0; j < U; ++j) x[j] = ldg_stream(v + b + lane + 32u * j);
 #pragma unroll
     for (int j = 0; j < U; ++j) m = fold4(m, x[j]);
+    if (stop && __ballot_sync(0xffffffffu, settles(m, is_power, thr))) return warp_max(m);
   }
   // one predicated batch for the remainder
-  if (i < nv) {
+  if (b < nv) {
     float4 x[U];
 #pragma unroll
     for (int j = 0; j < U; ++j) {
-      const uint32_t k = i + 32u * j;
+      const uint32_t k = b + lane + 32u * j;
       x[j] = make_float4(nan_f(), nan_f(), nan_f(), nan_f());
       if (k < nv) x[j] = ldg_stream(v + k);
     }
 #pragma unroll
     for (int j = 0; j < U; ++j) m = fold4(m, x[j]);
+    if (stop && __ballot_sync(0xffffffffu, settles(m, is_power, thr))) return warp_max(m);
   }
   const uint32_t done = head + nv * 4u;
   if (done + lane < T) m = fmaxf(m, __ldg(row + done + lane));
@@ -633,6 +659,7 @@ __global__ void __launch_bounds__(WARPS * 32) k_reduce_ldg(ReduceParams p) {
   TL_MARK(0);
   pdl_launch_dependents();
   const uint32_t n_mine = cta_row_count(p.total_rows);
+  const bool stop = rows_may_stop(p);
   if (threadIdx.x == 0) s_next = WARPS;
   __syncthreads();
   uint32_t j = warp;
@@ -640,7 +667,8 @@ __global__ void __launch_bounds__(WARPS * 32) k_reduce_ldg(ReduceParams p) {
   while (j < n_mine) {
     uint32_t seg, local;
     const float* row = row_ptr(p, blockIdx.x + j * gridDim.x, seg, local);
-    const float m = row_max_ldg<U>(row, p.T, lane);
+    const bool is_power = seg ? p.seg[1].is_power != 0 : p.seg[0].is_power != 0;
+    const float m = row_max_ldg<U>(row, p.T, lane, stop, is_power, p.thr);
     if (lane == 0) {
       if (!scratch_ok) wait_scratch_free(p), scratch_ok = true;
       publish_row(p, seg, local, m);
@@ -730,7 +758,7 @@ __global__ void __launch_bounds__(WARPS * 32) k_reduce_u8(ReduceParams p) {
       const uint8_t* row = reinterpret_cast<const uint8_t*>(p.seg[0].base) + (size_t)local * p.ld;
       m = row_max_u8<U>(row, p.T, lane, p.seg[0].smax != nullptr);
     } else {
-      m = row_max_ldg<U>(frow, p.T, lane);
+      m = row_max_ldg<U>(frow, p.T, lane, false, false, 0.0f);   // (byte-window calls read every row whole)
     }
     if (lane == 0) {
       if (!scratch_ok) wait_scratch_free(p), scratch_ok = true;
@@ -793,89 +821,117 @@ __device__ __forceinline__ uint64_t l2_evict_first_policy() {
 #ifndef GPR_TMA_LAYOUT_DEFINED
 #define GPR_TMA_LAYOUT_DEFINED
 struct TmaLayout {
-  uint32_t depth;         // stages per warp
+  uint32_t depth;         // stages per warp = rows in flight per warp
   uint32_t stage_bytes;   // capacity of one stage (multiple of 128)
-  uint32_t chunk_elems;   // elements copied per chunk (multiple of 4); a row = n_chunks chunks
+  uint32_t chunk_elems;   // elements copied per chunk (multiple of 4); a row read whole = n_chunks chunks
   uint32_t n_chunks;
+  uint32_t head_elems;    // elements of a row's first copy when the row may stop early (multiple of 4, <= chunk_elems)
 };
 #endif
 
 // Requirements (checked on the host): every row base 16-byte aligned, T % 4 == 0.
 //
 // Every warp runs its own TMA pipeline: a private ring of `depth` stages, each with one
-// mbarrier.  Lane 0 issues a 1-D bulk copy (row chunk -> stage) with the byte count expected on
-// the stage's barrier; the warp waits for the bytes, folds the chunk out of shared memory with
-// conflict-free 128-bit LDS, and — once every lane has finished reading — lane 0 immediately
-// re-arms the same stage with the chunk `depth` items ahead.  No producer warp, no empty
-// barriers, no cross-warp synchronisation: a stage is only ever touched by its owner warp, so
-// the mbarrier phase parity cannot alias, and NW * depth * chunk bytes stay in flight per SM
-// without holding a single register.
-// The CTA owns rows b, b + grid, ... (see k_reduce_ldg); its j-th row belongs to warp j % NW.
+// mbarrier, and each carrying one row with exactly one bulk copy in flight.  A row's copies are
+// its head (elements [0, h)) and then chunks of chunk_elems: copy c >= 1 covers
+// [h + (c - 1) chunk_elems, ...).  h = head_elems when rows may stop early, else chunk_elems (the
+// row is then cut exactly as n_chunks chunks).  Lane 0 issues a 1-D bulk copy with the byte count
+// expected on the stage's barrier; the warp visits the stages in ring order, waits for the bytes,
+// folds them out of shared memory with conflict-free 128-bit LDS into the row's running max and,
+// once every lane has finished reading, lane 0 re-arms the same stage: with the row's next chunk
+// if the row is neither finished nor settled, else — after publishing the row — with the head of
+// the next row the CTA hands out.  A copy is requested only after the row's previous copy has
+// been examined, so the bytes a row costs depend on nothing but its data and the layout, and no
+// copy is ever issued that would not be consumed.  No producer warp, no empty barriers: a stage
+// is only ever touched by its owner warp, so the mbarrier phase parity cannot alias.
+// The CTA owns rows b, b + grid, ... (see k_reduce_ldg); its first NW * depth rows start the
+// stages, the rest are handed out through a counter behind the barriers in shared memory, since
+// rows now cost anything from a head to a full read.
 template <int NW>
 __global__ void __launch_bounds__(NW * 32) k_reduce_tma(ReduceParams p, TmaLayout L) {
   extern __shared__ __align__(128) unsigned char smem[];
   const int lane = threadIdx.x & 31;
   const uint32_t w = threadIdx.x >> 5;
-  const uint32_t D = L.depth;
+  const uint32_t D = L.depth;  // <= 32: lane s keeps the row state of stage s
   unsigned char* stage0 = smem + (size_t)w * D * L.stage_bytes;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)NW * D * L.stage_bytes) + w * D;
+  uint64_t* const bars = reinterpret_cast<uint64_t*>(smem + (size_t)NW * D * L.stage_bytes);
+  uint64_t* full = bars + w * D;
+  unsigned int* next_row = reinterpret_cast<unsigned int*>(bars + NW * D);
 
   pdl_launch_dependents();
   const uint32_t n_rows = cta_row_count(p.total_rows);
-  const uint32_t my_rows = n_rows > w ? (uint32_t)(((uint64_t)n_rows - w + NW - 1) / NW) : 0u;  // (grid 1: n_rows ~ 2^32)
+  const bool stop = rows_may_stop(p);
+  const uint32_t h = stop ? L.head_elems : L.chunk_elems;
   bool scratch_ok = false;
-  const uint32_t n_items = my_rows * L.n_chunks;
 
   if (lane == 0) {
     for (uint32_t s = 0; s < D; ++s) mbar_init(&full[s], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncwarp();
+  if (threadIdx.x == 0) *next_row = NW * D;
+  __syncthreads();
   const uint64_t pol = l2_evict_first_policy();
 
-  // producer cursor (tracked by every lane, acted on by lane 0)
-  uint32_t pi = 0, pc = 0, pst = 0, issued = 0;
-  auto issue = [&]() {
+  // copy c of the CTA's j-th row into stage s (called by every lane, acted on by lane 0)
+  auto issue = [&](uint32_t s, uint32_t j, uint32_t c) {
     uint32_t seg, local;
-    const float* row = row_ptr(p, blockIdx.x + (w + NW * pi) * gridDim.x, seg, local);
-    const uint32_t e0 = pc * L.chunk_elems;
-    const uint32_t bytes = min(L.chunk_elems, p.T - e0) * 4u;
+    const float* row = row_ptr(p, blockIdx.x + j * gridDim.x, seg, local);
+    const uint32_t e0 = c ? h + (c - 1u) * L.chunk_elems : 0u;
+    const uint32_t bytes = min(c ? L.chunk_elems : h, p.T - e0) * 4u;
     if (lane == 0) {
-      mbar_expect_tx(&full[pst], bytes);
-      tma_load_1d(stage0 + (size_t)pst * L.stage_bytes, row + e0, bytes, &full[pst], pol);
+      mbar_expect_tx(&full[s], bytes);
+      tma_load_1d(stage0 + (size_t)s * L.stage_bytes, row + e0, bytes, &full[s], pol);
     }
-    if (++pc == L.n_chunks) pc = 0, ++pi;
-    if (++pst == D) pst = 0;
-    ++issued;
   };
-  while (issued < D && issued < n_items) issue();
+  // stage s's row (CTA-local index, >= n_rows: the stage is drained), its next copy and running max, kept by lane s
+  uint32_t my_j = min(w + NW * (uint32_t)lane, n_rows), my_c = 0;
+  float my_m = nan_f();
+  uint32_t live = 0;
+  for (uint32_t s = 0; s < D; ++s) {
+    const uint32_t j = w + NW * s;
+    if (j < n_rows) issue(s, j, 0u), ++live;
+  }
 
-  uint32_t cs = 0, cph = 0;
-  for (uint32_t i = 0; i < my_rows; ++i) {
+  uint32_t phase = 0;  // bit s: parity of stage s's next completion
+  for (uint32_t s = 0; live; s = s + 1u == D ? 0u : s + 1u) {
+    uint32_t j = __shfl_sync(0xffffffffu, my_j, (int)s);
+    if (j >= n_rows) continue;
+    uint32_t c = __shfl_sync(0xffffffffu, my_c, (int)s);
+    float m = __uint_as_float(__shfl_sync(0xffffffffu, __float_as_uint(my_m), (int)s));
+    mbar_wait(&full[s], (phase >> s) & 1u);
+    phase ^= 1u << s;
+    const uint32_t e0 = c ? h + (c - 1u) * L.chunk_elems : 0u;
+    const uint32_t n = min(c ? L.chunk_elems : h, p.T - e0);
+    const float4* v = reinterpret_cast<const float4*>(stage0 + (size_t)s * L.stage_bytes);
+    const uint32_t nv = n >> 2;
     float m0 = nan_f(), m1 = nan_f();
-    for (uint32_t c = 0; c < L.n_chunks; ++c) {
-      mbar_wait(&full[cs], cph);
-      const float4* v = reinterpret_cast<const float4*>(stage0 + (size_t)cs * L.stage_bytes);
-      const uint32_t nv = min(L.chunk_elems, p.T - c * L.chunk_elems) >> 2;
-      uint32_t k = lane;
+    uint32_t k = lane;
 #pragma unroll 4
-      for (; k + 32u < nv; k += 64u) {
-        const float4 a = v[k], b = v[k + 32u];
-        m0 = fold4(m0, a);
-        m1 = fold4(m1, b);
+    for (; k + 32u < nv; k += 64u) {
+      const float4 a = v[k], b = v[k + 32u];
+      m0 = fold4(m0, a);
+      m1 = fold4(m1, b);
+    }
+    if (k < nv) m0 = fold4(m0, v[k]);
+    m = fmaxf(m, warp_max(fmaxf(m0, m1)));
+    __syncwarp();  // every lane has its data in registers: the stage may be overwritten
+    uint32_t seg, local;
+    (void)row_ptr(p, blockIdx.x + j * gridDim.x, seg, local);
+    const bool is_power = seg ? p.seg[1].is_power != 0 : p.seg[0].is_power != 0;
+    if (e0 + n < p.T && !(stop && settles(m, is_power, p.thr))) {
+      issue(s, j, ++c);
+    } else {
+      uint32_t next = 0;
+      if (lane == 0) {
+        if (!scratch_ok) wait_scratch_free(p), scratch_ok = true;
+        publish_row(p, seg, local, m);
+        next = atomicAdd(next_row, 1u);
       }
-      if (k < nv) m0 = fold4(m0, v[k]);
-      __syncwarp();  // every lane has its data in registers: the stage may be overwritten
-      if (issued < n_items) issue();
-      if (++cs == D) cs = 0, cph ^= 1u;
+      j = min(__shfl_sync(0xffffffffu, next, 0), n_rows), c = 0, m = nan_f();
+      if (j < n_rows) issue(s, j, 0u);
+      else --live;
     }
-    const float m = warp_max(fmaxf(m0, m1));
-    if (lane == 0) {
-      uint32_t seg, local;
-      (void)row_ptr(p, blockIdx.x + (w + NW * i) * gridDim.x, seg, local);
-      if (!scratch_ok) wait_scratch_free(p), scratch_ok = true;
-      publish_row(p, seg, local, m);
-    }
+    if ((uint32_t)lane == s) my_j = j, my_c = c, my_m = m;
   }
 }
 

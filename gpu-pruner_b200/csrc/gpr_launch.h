@@ -20,15 +20,20 @@ constexpr int kLdgWarps = 16;     // k_reduce_ldg / k_reduce_u8: warps per CTA
 constexpr int kLdgUnroll = 8;     // k_reduce_ldg: 16-byte loads per lane in flight
 constexpr int kU8Unroll = 4;      // k_reduce_u8: 16-byte loads per lane in flight
 constexpr size_t kTmaSmemBudget = 208 * 1024;
+// k_reduce_tma: samples in the first copy of a row (multiple of 4).  Most busy rows are settled by their first
+// sample, so the head is all that is read of them; a row the head does not settle is read on in chunk_elems chunks.
+constexpr uint32_t kTmaHeadElems = 128;
+constexpr uint32_t kTmaMaxDepth = 32;   // k_reduce_tma keeps the row of stage s in lane s
 
 // (the same definition, under the same guard, is in gpr_kernels.cuh's namespace body, which must also compile alone)
 #ifndef GPR_TMA_LAYOUT_DEFINED
 #define GPR_TMA_LAYOUT_DEFINED
 struct TmaLayout {
-  uint32_t depth;         // stages per warp
+  uint32_t depth;         // stages per warp = rows in flight per warp
   uint32_t stage_bytes;   // capacity of one stage (multiple of 128)
-  uint32_t chunk_elems;   // elements copied per chunk (multiple of 4); a row = n_chunks chunks
+  uint32_t chunk_elems;   // elements copied per chunk (multiple of 4); a row read whole = n_chunks chunks
   uint32_t n_chunks;
+  uint32_t head_elems;    // elements of a row's first copy when the row may stop early (multiple of 4, <= chunk_elems)
 };
 #endif
 
@@ -69,13 +74,15 @@ inline TmaLayout tma_layout(const LaunchKnobs& k, uint32_t T, int nw) {
   L.n_chunks = (T + ce - 1) / ce;
   L.stage_bytes = (ce * 4u + 127u) & ~127u;
   uint32_t d = (uint32_t)((kTmaSmemBudget - 1024) / ((size_t)L.stage_bytes * nw));
-  d = std::min<uint32_t>(d, (uint32_t)k.tma_depth_max);
+  d = std::min<uint32_t>(d, std::min<uint32_t>((uint32_t)k.tma_depth_max, kTmaMaxDepth));
   L.depth = std::max<uint32_t>(d, 1u);
+  L.head_elems = std::min<uint32_t>(kTmaHeadElems, ce);
   return L;
 }
 
+// stages, one mbarrier per stage, and the CTA's row counter
 inline size_t tma_smem_bytes(const TmaLayout& L, int nw) {
-  return (size_t)nw * L.depth * L.stage_bytes + (size_t)nw * L.depth * sizeof(uint64_t);
+  return (size_t)nw * L.depth * L.stage_bytes + (size_t)nw * L.depth * sizeof(uint64_t) + sizeof(uint64_t);
 }
 
 // The reduce launch for `total_rows` rows of T samples.  tma_ok: every row base is 16-byte aligned and T % 4 == 0
