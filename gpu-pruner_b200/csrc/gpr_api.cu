@@ -26,6 +26,7 @@
 #include <vector>
 
 #include "gpr_kernels.cuh"
+#include "gpr_groups.cuh"
 #include "gpr_ring.cuh"
 #include "gpr_synth.cuh"
 #include "gpr_text_kernels.cuh"
@@ -139,10 +140,22 @@ struct gpr_ctx {
   size_t gather_cap = 0;
   float* d_smax = nullptr;
   size_t smax_cap = 0;
+  // `sum by` groups (gpr_window.groups, gpr_groups.cuh): single-buffered, so a decision with a table runs without PDL
+  uint32_t* d_grouped = nullptr;   // [P][MW] rows of groups of two or more
+  size_t grouped_cap = 0;
+  uint32_t* d_gpods = nullptr;     // [1 + P]: count, then the pods with such groups
+  size_t gpods_cap = 0;
+  float* d_gmax = nullptr;         // [P*G] max of the grouped rows when the caller did not ask for series_max
+  size_t gmax_cap = 0;
+  uint32_t* d_gtable = nullptr;    // [P*G] a host table, uploaded
+  size_t gtable_cap = 0;
+  uint32_t* d_islots = nullptr;    // [P][MW] idle_slots for host outputs
+  size_t islots_cap = 0;
+  unsigned int* h_gerr = nullptr;  // host-mapped: 1 + a pod whose device group table is malformed
   unsigned long long* h_counts = nullptr;  // pinned [kSlots][4]: n_series, n_candidates, n_decisions,
                                            // %globaltimer at completion; then [mark, error word]
   unsigned long long* h_mark = nullptr;    // %globaltimer written by the last gpr_timer_begin
-  unsigned int* h_err = nullptr;           // raised by a kernel whose peer wait timed out
+  unsigned int* h_err = nullptr;           // raised by a kernel whose peer wait timed out (h_gerr is the next word)
   std::vector<Pending> pending;
   std::vector<uint64_t> stamps;            // completion stamps of the decisions retired by the last gpr_sync
   std::vector<uint64_t> phase_stamps;      // 4 per decision: fold start, folded, flags raised, peers arrived
@@ -312,33 +325,37 @@ cudaError_t launch_ex(Kernel k, uint32_t grid, uint32_t block, size_t smem, cuda
   return cudaLaunchKernelEx(&cfg, k, args...);
 }
 
-template <int NW>
+template <int NW, bool kGroups>
 cudaError_t launch_tma(gpr_ctx* ctx, const gpr::ReduceParams& rp, const gpr::ReducePlan& plan, bool pdl) {
-  return launch_ex(gpr::k_reduce_tma<NW>, plan.grid, plan.block, plan.smem, ctx->stream, pdl, rp, plan.L);
+  return launch_ex(gpr::k_reduce_tma<NW, kGroups>, plan.grid, plan.block, plan.smem, ctx->stream, pdl, rp, plan.L);
 }
 
-// launch one reduce pass over the rows described by rp
-int launch_reduce(gpr_ctx* ctx, gpr::ReduceParams& rp, bool tma_ok, bool pdl) {
+// launch one reduce pass over the rows described by rp (kGroups: the instantiation for a group table)
+template <bool kGroups>
+int launch_reduce_as(gpr_ctx* ctx, gpr::ReduceParams& rp, bool tma_ok, bool pdl) {
   if (rp.total_rows == 0) return GPR_OK;
   // AUTO = the TMA pipeline (measured winner on H100 at C2 and C3, DESIGN.md §4.3); rows that are
   // not 16-byte aligned or have T % 4 != 0 cannot be bulk-copied and take the LDG kernel
   const gpr::ReducePlan plan = gpr::plan_reduce(launch_knobs(ctx), rp.T, rp.total_rows, tma_ok, rp.util_u8 != 0);
   cudaError_t e;
   if (plan.kernel == gpr::kReduceU8) {
-    e = launch_ex(gpr::k_reduce_u8<kLdgWarps, gpr::kU8Unroll>, plan.grid, plan.block, 0, ctx->stream, pdl, rp);
+    e = launch_ex(gpr::k_reduce_u8<kLdgWarps, gpr::kU8Unroll, kGroups>, plan.grid, plan.block, 0, ctx->stream, pdl, rp);
   } else if (plan.kernel == gpr::kReduceTma) {
     const int nw = ctx->tma_warps;
-    if (nw == 4) e = launch_tma<4>(ctx, rp, plan, pdl);
-    else if (nw == 16) e = launch_tma<16>(ctx, rp, plan, pdl);
-    else if (nw == 32) e = launch_tma<32>(ctx, rp, plan, pdl);
-    else e = launch_tma<8>(ctx, rp, plan, pdl);
+    if (nw == 4) e = launch_tma<4, kGroups>(ctx, rp, plan, pdl);
+    else if (nw == 16) e = launch_tma<16, kGroups>(ctx, rp, plan, pdl);
+    else if (nw == 32) e = launch_tma<32, kGroups>(ctx, rp, plan, pdl);
+    else e = launch_tma<8, kGroups>(ctx, rp, plan, pdl);
   } else {
-    e = launch_ex(gpr::k_reduce_ldg<kLdgWarps, kLdgUnroll>, plan.grid, plan.block, 0, ctx->stream, pdl, rp);
+    e = launch_ex(gpr::k_reduce_ldg<kLdgWarps, kLdgUnroll, kGroups>, plan.grid, plan.block, 0, ctx->stream, pdl, rp);
   }
   ctx->launches++;
   CU(e);
   CU(cudaGetLastError());
   return GPR_OK;
+}
+int launch_reduce(gpr_ctx* ctx, gpr::ReduceParams& rp, bool tma_ok, bool pdl) {
+  return rp.grouped ? launch_reduce_as<true>(ctx, rp, tma_ok, pdl) : launch_reduce_as<false>(ctx, rp, tma_ok, pdl);
 }
 
 int copy_rows_h2d(gpr_ctx* ctx, void* dst, const void* src, size_t n_rows, uint32_t T,
@@ -362,9 +379,14 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
   if (!ctx) return GPR_E_INVALID;
   NvtxRange nvtx_range(resident ? "gpr_decide_resident" : "gpr_decide");
   if (!win || !res) return fail(ctx, GPR_E_INVALID, "window/result is NULL");
-  if (win->struct_size != sizeof(gpr_window) || res->struct_size != sizeof(gpr_result))
-    return fail(ctx, GPR_E_INVALID, "struct_size mismatch (window %u/%zu result %u/%zu)",
-                win->struct_size, sizeof(gpr_window), res->struct_size, sizeof(gpr_result));
+  // a caller built before gpr_window.groups / gpr_result.idle_slots existed passes the older sizes: no such fields
+  const size_t win_v1 = offsetof(gpr_window, groups), res_v1 = offsetof(gpr_result, idle_slots);
+  if ((win->struct_size != sizeof(gpr_window) && win->struct_size != win_v1) ||
+      (res->struct_size != sizeof(gpr_result) && res->struct_size != res_v1))
+    return fail(ctx, GPR_E_INVALID, "struct_size mismatch (window %u/%zu or %zu, result %u/%zu or %zu)",
+                win->struct_size, sizeof(gpr_window), win_v1, res->struct_size, sizeof(gpr_result), res_v1);
+  const uint32_t* const groups = win->struct_size == sizeof(gpr_window) ? win->groups : nullptr;
+  uint32_t* const idle_slots = res->struct_size == sizeof(gpr_result) ? res->idle_slots : nullptr;
   CU(cudaSetDevice(ctx->device));
 
   uint32_t P = win->n_pods, G = win->n_gpus, T = win->n_samples;
@@ -418,6 +440,19 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
     return fail(ctx, GPR_E_INVALID, "with a communicator n_pods must be a multiple of 32 (got %u)", P);
   if ((int)ctx->pending.size() >= kSlots)
     return fail(ctx, GPR_E_STATE, "too many outstanding async results; call gpr_sync");
+  // a host group table is checked here, before anything is enqueued (a device table by k_group_rows)
+  const bool grouped = groups != nullptr && P > 0;
+  if (grouped && in_kind == GPR_MEM_HOST) {
+    for (uint32_t p = 0; p < P; ++p) {
+      const uint32_t* e = groups + (size_t)p * G;
+      for (uint32_t g = 0; g < G; ++g) {
+        const uint32_t x = e[g], l = x & gpr::kGroupLeader;
+        if ((x & ~(gpr::kGroupLeader | gpr::kGroupUtil)) != 0u || l > g || (e[l] & gpr::kGroupLeader) != l)
+          return fail(ctx, GPR_E_INVALID, "gpr_window.groups: malformed entry 0x%x at pod %u slot %u (leader above its "
+                      "slot, a leader that does not lead itself, or bits other than 0-7 and GPR_GROUP_UTIL)", x, p, g);
+      }
+    }
+  }
 
   if (host_in) {
     // staging is dense, so only the number of cells matters: a window with one more GPU slot or a few more
@@ -456,6 +491,15 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
   if (want_smax && host_out &&
       (rc = grow(ctx, &ctx->d_smax, &ctx->smax_cap, (size_t)S + 4)) != GPR_OK)
     return rc;
+  if (idle_slots && host_out && (rc = grow(ctx, &ctx->d_islots, &ctx->islots_cap, (size_t)P * MW + 4)) != GPR_OK)
+    return rc;
+  if (grouped) {
+    if ((rc = grow(ctx, &ctx->d_grouped, &ctx->grouped_cap, (size_t)P * MW + 4)) != GPR_OK ||
+        (rc = grow(ctx, &ctx->d_gpods, &ctx->gpods_cap, (size_t)P + 4)) != GPR_OK ||
+        (!want_smax && (rc = grow(ctx, &ctx->d_gmax, &ctx->gmax_cap, (size_t)S + 4)) != GPR_OK) ||
+        (in_kind == GPR_MEM_HOST && (rc = grow(ctx, &ctx->d_gtable, &ctx->gtable_cap, (size_t)S + 4)) != GPR_OK))
+      return rc;
+  }
 
   // ---- gates -----------------------------------------------------------------------------
   const uint8_t* d_elig = win->eligible;
@@ -502,6 +546,7 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
   // (a series_max target also tells the reduce kernels to read every row whole: the true max is an output; without
   // one they stop reading a row at the first sample that settles its flag, gpr_kernels.cuh "early exit")
   float* smax_dev = want_smax ? (host_out ? ctx->d_smax : res->series_max) : nullptr;
+  uint32_t* islots_dev = idle_slots ? (host_out ? ctx->d_islots : idle_slots) : nullptr;
 
   gpr::FoldParams fp;
   fp.idle_mask = masks;
@@ -533,6 +578,7 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
   fp.poll_ns = ctx->poll_ns;
   fp.my_ll = nullptr;
   fp.late_order = 0;
+  fp.islots = islots_dev;
   for (int r = 0; r < gpr::kMaxPeers; ++r) fp.peer_ll[r] = nullptr;
   if (fused) {
     fp.exchange_debug = ctx->exchange_debug;
@@ -547,8 +593,9 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
       for (int r = 0; r < ctx->world; ++r)
         fp.peer_ll[r] = reinterpret_cast<unsigned long long*>(ctx->p2p_peer[r] + ctx->p2p_ll_off[xset]);
       fp.my_ll = reinterpret_cast<unsigned long long*>(ctx->p2p_block + ctx->p2p_ll_off[xset]);
-      // (veto bits go straight to the caller's buffer from every fold CTA, so that call keeps the early wait)
-      fp.late_order = ctx->exchange_late && vbits_dev == nullptr ? 1 : 0;
+      // (veto bits and idle_slots go straight to the caller's buffers from every fold CTA, so such a call keeps the
+      // early wait)
+      fp.late_order = ctx->exchange_late && vbits_dev == nullptr && islots_dev == nullptr ? 1 : 0;
     }
     fp.step = ++ctx->p2p_step;
     fp.out_dbits = host_out ? nullptr : res->decision_bits;
@@ -570,6 +617,47 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
   const uint32_t fold_threads = (uint32_t)ctx->fold_threads;
   const uint32_t fold_grid = gpr::fold_grid(launch_knobs(ctx), P);
 
+  // ---- `sum by` groups: the table's kernels around the reduce (gpr_groups.cuh) -----------------
+  gpr::GroupParams gq;
+  memset(&gq, 0, sizeof gq);
+  if (grouped) {
+    gq.table = groups;
+    if (in_kind == GPR_MEM_HOST) {
+      CU(cudaMemcpyAsync(ctx->d_gtable, groups, (size_t)S * 4u, cudaMemcpyHostToDevice, ctx->stream));
+      gq.table = ctx->d_gtable;
+    }
+    gq.need = ctx->d_grouped;
+    gq.n_pods = ctx->d_gpods;
+    gq.pods = ctx->d_gpods + 1;
+    gq.gmax = want_smax ? smax_dev : ctx->d_gmax;
+    gq.idle_mask = masks;
+    gq.bad = ctx->h_gerr;
+    gq.P = P, gq.G = G, gq.mw = MW;
+    rp.grouped = ctx->d_grouped;
+    rp.gmax = ctx->d_gmax;
+    ctx->last_was_reduce = false;   // the group scratch is single-buffered: no PDL into or out of this decision
+  }
+  const uint32_t group_grid = gpr::group_grid(launch_knobs(ctx), P);
+  auto launch_group_rows = [&]() -> int {
+    CU(cudaMemsetAsync(ctx->d_gpods, 0, sizeof(uint32_t), ctx->stream));
+    CU(launch_ex(gpr::k_group_rows, group_grid, gpr::kGroupBlock, 0, ctx->stream, false, gq));
+    ctx->launches++;
+    return GPR_OK;
+  };
+  auto launch_group_sum = [&]() -> int {
+    CU(launch_ex(gpr::k_group_sum, group_grid, gpr::kGroupBlock, 0, ctx->stream, false, gq));
+    ctx->launches++;
+    return GPR_OK;
+  };
+  const bool fold_pdl = can_pdl && !grouped;
+  auto launch_fold = [&](bool pdl) -> cudaError_t {
+    if (fused)
+      return islots_dev ? launch_ex(gpr::k_fold<true, true>, fold_grid, fold_threads, 0, ctx->stream, pdl, fp)
+                        : launch_ex(gpr::k_fold<true, false>, fold_grid, fold_threads, 0, ctx->stream, pdl, fp);
+    return islots_dev ? launch_ex(gpr::k_fold<false, true>, fold_grid, fold_threads, 0, ctx->stream, pdl, fp)
+                      : launch_ex(gpr::k_fold<false, false>, fold_grid, fold_threads, 0, ctx->stream, pdl, fp);
+  };
+
   if (!async) {
     CU(cudaEventRecord(ctx->ev_k0, ctx->stream));
     ctx->last_was_reduce = false;
@@ -589,13 +677,15 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
       // when that is provably safe: our own stream (no foreign producer kernels between), the
       // newest op on it is one of our fold kernels, and this launch writes nothing but its own
       // scratch set (series_max would go straight to the caller's buffer).
-      const bool pdl = can_pdl && ctx->last_was_reduce && !want_smax;
+      // (nor with a group table: k_group_rows writes the table's single-buffered scratch)
+      const bool pdl = can_pdl && ctx->last_was_reduce && !want_smax && !grouped;
+      if (grouped && (rc = launch_group_rows()) != GPR_OK) return rc;
       if ((rc = launch_reduce(ctx, rp, tma_ok, pdl)) != GPR_OK) return rc;
-      CU(fused ? launch_ex(gpr::k_fold<true>, fold_grid, fold_threads, 0, ctx->stream, can_pdl, fp)
-               : launch_ex(gpr::k_fold<false>, fold_grid, fold_threads, 0, ctx->stream, can_pdl, fp));
+      if (grouped && (rc = launch_group_sum()) != GPR_OK) return rc;
+      CU(launch_fold(fold_pdl));
       ctx->launches++;
       ctx->uses[sset]++;
-      ctx->last_was_reduce = true;
+      ctx->last_was_reduce = !grouped;
     }
   } else {
     // ---- host window: pod chunks, H2D on the copy stream overlapped with the reduce --------
@@ -611,6 +701,7 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
     const bool tma_ok = (T % 4u) == 0;
     const char* util_bytes = reinterpret_cast<const char*>(util);
     char* stage_bytes = reinterpret_cast<char*>(ctx->d_util_stage);
+    if (grouped && (rc = launch_group_rows()) != GPR_OK) return rc;
     for (uint32_t c = 0; c < n_chunks; ++c) {
       const uint32_t p0 = c * chunk_pods, p1 = std::min(P, p0 + chunk_pods);
       const size_t row0 = (size_t)p0 * G, n_rows = (size_t)(p1 - p0) * G;
@@ -633,11 +724,12 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
       rp.seg[1] = gpr::Segment{dp, masks + ((size_t)P + p0) * MW, nullptr,
                                use_power ? (uint32_t)n_rows : 0u, 1u};
       rp.total_rows = (uint32_t)n_rows * (use_power ? 2u : 1u);
+      if (grouped) rp.grouped = ctx->d_grouped + (size_t)p0 * MW, rp.gmax = ctx->d_gmax ? ctx->d_gmax + row0 : nullptr;
       if ((rc = launch_reduce(ctx, rp, tma_ok, false)) != GPR_OK) return rc;
     }
+    if (grouped && (rc = launch_group_sum()) != GPR_OK) return rc;
     if (P > 0) {
-      CU(fused ? launch_ex(gpr::k_fold<true>, fold_grid, fold_threads, 0, ctx->stream, false, fp)
-               : launch_ex(gpr::k_fold<false>, fold_grid, fold_threads, 0, ctx->stream, false, fp));
+      CU(launch_fold(false));
       ctx->launches++;
       ctx->uses[sset]++;
     }
@@ -682,6 +774,8 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
   if (want_smax && host_out && S > 0)
     CU(cudaMemcpyAsync(res->series_max, ctx->d_smax, (size_t)S * 4u, cudaMemcpyDeviceToHost,
                        ctx->stream));
+  if (idle_slots && host_out && P > 0)
+    CU(cudaMemcpyAsync(idle_slots, ctx->d_islots, (size_t)P * MW * 4u, cudaMemcpyDeviceToHost, ctx->stream));
   ctx->pending.push_back(Pending{res, slot});
   res->kernel_ms = 0.0;
   return GPR_OK;
@@ -706,11 +800,18 @@ int sync_impl(gpr_ctx* ctx) {
     for (int k = 4; k < 8; ++k) ctx->phase_stamps.push_back(c[k]);
   }
   ctx->pending.clear();
+  const unsigned int gerr = *ctx->h_gerr;
+  *ctx->h_gerr = 0;
   if (*ctx->h_err) {
     *ctx->h_err = 0;
     ctx->masks_dirty = true;
     return fail(ctx, GPR_E_STATE, "a peer rank never arrived at the bitmap exchange / rendezvous (waited %llu s); "
                 "the results of this batch are not global", gpr::kPeerTimeoutNs / 1000000000ull);
+  }
+  if (gerr) {
+    ctx->masks_dirty = true;
+    return fail(ctx, GPR_E_INVALID, "gpr_window.groups: malformed device group table at pod %u (leader above its slot, "
+                "a leader that does not lead itself, or bits other than 0-7 and GPR_GROUP_UTIL)", gerr - 1u);
   }
   return GPR_OK;
 }
@@ -889,7 +990,8 @@ void gpr_destroy(gpr_ctx* ctx) {
                  ctx->d_flush,      ctx->d_res_util,    ctx->d_res_power,  ctx->d_cols,
                  ctx->d_idx_util,   ctx->d_idx_power,   ctx->d_text[0],    ctx->d_text[1],
                  ctx->d_text[2],    ctx->d_marks,       ctx->d_mark_counts, ctx->d_spans,
-                 ctx->d_tplane[0],  ctx->d_tplane[1]};
+                 ctx->d_tplane[0],  ctx->d_tplane[1],  ctx->d_grouped,   ctx->d_gpods,
+                 ctx->d_gmax,       ctx->d_gtable,     ctx->d_islots};
   for (void* p : dev)
     if (p) cudaFree(p);
   if (ctx->h_counts) cudaFreeHost(ctx->h_counts);
@@ -990,6 +1092,7 @@ int gpr_create(const gpr_config* cfg, gpr_ctx** out) {
     memset(c->h_counts, 0, ((size_t)kSlots * 8 + 2) * sizeof(unsigned long long));
     c->h_mark = c->h_counts + (size_t)kSlots * 8;
     c->h_err = reinterpret_cast<unsigned int*>(c->h_mark + 1);
+    c->h_gerr = c->h_err + 1;
     c->pending.reserve(kSlots);
     c->stamps.reserve(kSlots);
 
@@ -1015,6 +1118,15 @@ int gpr_create(const gpr_config* cfg, gpr_ctx** out) {
     CU(cudaFuncSetAttribute(gpr::k_reduce_tma<16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             (int)kTmaSmemBudget));
     CU(cudaFuncSetAttribute(gpr::k_reduce_tma<32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)kTmaSmemBudget));
+    // (the instantiations for calls with a `sum by` group table)
+    CU(cudaFuncSetAttribute(gpr::k_reduce_tma<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)kTmaSmemBudget));
+    CU(cudaFuncSetAttribute(gpr::k_reduce_tma<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)kTmaSmemBudget));
+    CU(cudaFuncSetAttribute(gpr::k_reduce_tma<16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)kTmaSmemBudget));
+    CU(cudaFuncSetAttribute(gpr::k_reduce_tma<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             (int)kTmaSmemBudget));
 
     c->max_pods = cfg->max_pods, c->max_gpus = cfg->max_gpus, c->max_samples = cfg->max_samples;

@@ -99,6 +99,8 @@ struct FoldParams {
   // reduce n + 4), which saw every peer's step n + 2 words, which a peer sends only after its reduce n + 2 ran, which
   // waited for that peer's fold n — so nobody still polls for step n when its slots are overwritten.
   int late_order;
+  uint32_t* islots;                      // [P][mw] or nullptr: gpr_result.idle_slots, each pod's idle words before
+                                         // the fold clears them (this rank's pods)
 };
 
 // One rank's view of the exchange block header, for the stand-alone rendezvous (gpr_timer_begin)
@@ -122,6 +124,10 @@ struct ReduceParams {
   const unsigned long long* done;  // scratch-set guard, see wait_scratch_free
   unsigned long long need;
   uint32_t util_u8;   // seg[0] rows are biased bytes (GPR_FMT_U8B), k_reduce_u8 only
+  // group table (gpr_groups.cuh), or nullptr: bit g of word (local / G) * mw + g / 32 marks a util row of a `sum by`
+  // group of two or more.  Such a row is read whole and its max goes to gmax[local] (seg[0].smax when that is set).
+  const uint32_t* grouped;
+  float* gmax;
 };
 
 __device__ __forceinline__ unsigned long long gtime() {
@@ -478,8 +484,9 @@ __device__ __forceinline__ void exchange_bitmaps_ll(const FoldParams& f, uint32_
 // mask updates are visible.  Grid = a handful of CTAs (32 words each); the last one to finish
 // (ticket) performs the multi-GPU exchange, publishes the counters and releases the scratch set.
 // kExchange = false is the single-GPU instantiation: the exchange (and the registers its batched loads need) is
-// compiled out, so that path is the same code as before the exchange existed.
-template <bool kExchange>
+// compiled out, so that path is the same code as before the exchange existed.  kSlots: the call asked for
+// gpr_result.idle_slots (f.islots); without it that copy is compiled out too.
+template <bool kExchange, bool kSlots = false>
 __global__ void __launch_bounds__(256) k_fold(FoldParams f) {
   __shared__ unsigned long long s_cnt[3];
   __shared__ unsigned int s_last;
@@ -492,6 +499,20 @@ __global__ void __launch_bounds__(256) k_fold(FoldParams f) {
   const uint32_t gw = blockIdx.x * warps_per_cta + (threadIdx.x >> 5);
   const uint32_t n_words = (f.P + 31u) / 32u;
   unsigned long long a = 0, b = 0, c = 0;
+  if (kSlots) {
+    // each pod's idle words as they are (idle elements, before veto and gates), read by the warp that clears them
+    // in fold_words below: the same words in the same order.  idle_slots is the caller's buffer, like the bitmaps:
+    // the previous decision's fold may still be writing it, so the copy waits for that fold first (a call with
+    // idle_slots never takes the late output ordering).
+    if (threadIdx.x == 0) spin_until_gpu(f.prev_done, f.prev_need);
+    __syncthreads();
+    for (uint32_t w = gw; w < n_words; w += gridDim.x * warps_per_cta) {
+      const uint32_t pod = w * 32u + (uint32_t)lane;
+      if (pod < f.P)
+        for (uint32_t k = 0; k < f.mw; ++k)
+          f.islots[(size_t)pod * f.mw + k] = __ldcg(f.idle_mask + (size_t)pod * f.mw + k);
+    }
+  }
   fold_words<4>(f, gw, n_words, gridDim.x * warps_per_cta, lane, a, b, c);
   block_counts(s_cnt, a, b, c, lane);
   __syncthreads();  // (thread 0's fence below is cumulative over what the CTA stored before this barrier)
@@ -565,8 +586,15 @@ __device__ __forceinline__ uint32_t cta_row_count(uint32_t total_rows) {
 // before a warp's first publish: the decision that last used this scratch set must have folded
 __device__ __forceinline__ void wait_scratch_free(const ReduceParams& p) { spin_until_gpu(p.done, p.need); }
 
+// a util row of a `sum by` group of two or more (ReduceParams.grouped); without a table a uniform false
+__device__ __forceinline__ bool row_grouped(const ReduceParams& p, uint32_t seg, uint32_t local) {
+  if (p.grouped == nullptr || seg != 0u) return false;
+  const uint32_t g = local % p.G;
+  return (p.grouped[(size_t)(local / p.G) * p.mw + (g >> 5)] >> (g & 31u)) & 1u;
+}
+
 __device__ __forceinline__ void publish_row(const ReduceParams& p, uint32_t seg, uint32_t local,
-                                            float m) {
+                                            float m, bool grouped) {
   const bool is_power = seg ? p.seg[1].is_power != 0 : p.seg[0].is_power != 0;
   uint32_t* mask = seg ? p.seg[1].mask : p.seg[0].mask;
   float* smax = seg ? p.seg[1].smax : p.seg[0].smax;
@@ -578,6 +606,7 @@ __device__ __forceinline__ void publish_row(const ReduceParams& p, uint32_t seg,
     atomicOr(mask + (size_t)(local / p.G) * p.mw + (g >> 5), 1u << (g & 31u));
   }
   if (smax) smax[local] = m;
+  else if (grouped) p.gmax[local] = m;   // the group sum (k_group_sum) reads it
 }
 
 // ------------------------------------------------------------------------------------------
@@ -589,6 +618,7 @@ __device__ __forceinline__ void publish_row(const ReduceParams& p, uint32_t seg,
 // A row may stop being read at the first read sample that settles it, unless the call asks for
 // series_max: the true max is an output then, and every row is read in full.  An idle row — the
 // only kind n_series counts — is always read to its end, so every output is what a full read gives.
+// A row of a `sum by` group of two or more (row_grouped) is read in full too: its max is summed.
 __device__ __forceinline__ bool settles(float m, bool is_power, float thr) {
   return is_power ? m >= thr : m > 0.0f;
 }
@@ -648,7 +678,9 @@ __device__ __forceinline__ float row_max_ldg(const float* __restrict__ row, uint
   return warp_max(m);
 }
 
-template <int WARPS, int U>
+// kGroups: the instantiation for calls with a group table (ReduceParams.grouped); without one the kernel is compiled
+// without the per-row test, so the ungrouped path is the same code as before tables existed.
+template <int WARPS, int U, bool kGroups = false>
 __global__ void __launch_bounds__(WARPS * 32) k_reduce_ldg(ReduceParams p) {
   __shared__ unsigned int s_next;
   const int lane = threadIdx.x & 31;
@@ -668,10 +700,11 @@ __global__ void __launch_bounds__(WARPS * 32) k_reduce_ldg(ReduceParams p) {
     uint32_t seg, local;
     const float* row = row_ptr(p, blockIdx.x + j * gridDim.x, seg, local);
     const bool is_power = seg ? p.seg[1].is_power != 0 : p.seg[0].is_power != 0;
-    const float m = row_max_ldg<U>(row, p.T, lane, stop, is_power, p.thr);
+    const bool grouped = kGroups && row_grouped(p, seg, local);
+    const float m = row_max_ldg<U>(row, p.T, lane, stop && !grouped, is_power, p.thr);
     if (lane == 0) {
       if (!scratch_ok) wait_scratch_free(p), scratch_ok = true;
-      publish_row(p, seg, local, m);
+      publish_row(p, seg, local, m, grouped);
       j = atomicAdd(&s_next, 1u);
     }
     j = __shfl_sync(0xffffffffu, j, 0);
@@ -739,7 +772,7 @@ __device__ __forceinline__ float row_max_u8(const uint8_t* __restrict__ row, uin
   return (float)(m - 1u);
 }
 
-template <int WARPS, int U>
+template <int WARPS, int U, bool kGroups = false>
 __global__ void __launch_bounds__(WARPS * 32) k_reduce_u8(ReduceParams p) {
   __shared__ unsigned int s_next;
   const int lane = threadIdx.x & 31;
@@ -754,15 +787,16 @@ __global__ void __launch_bounds__(WARPS * 32) k_reduce_u8(ReduceParams p) {
     uint32_t seg, local;
     const float* frow = row_ptr(p, blockIdx.x + j * gridDim.x, seg, local);
     float m;
+    const bool grouped = kGroups && row_grouped(p, seg, local);
     if (seg == 0u && p.util_u8) {
       const uint8_t* row = reinterpret_cast<const uint8_t*>(p.seg[0].base) + (size_t)local * p.ld;
-      m = row_max_u8<U>(row, p.T, lane, p.seg[0].smax != nullptr);
+      m = row_max_u8<U>(row, p.T, lane, p.seg[0].smax != nullptr || grouped);
     } else {
       m = row_max_ldg<U>(frow, p.T, lane, false, false, 0.0f);   // (byte-window calls read every row whole)
     }
     if (lane == 0) {
       if (!scratch_ok) wait_scratch_free(p), scratch_ok = true;
-      publish_row(p, seg, local, m);
+      publish_row(p, seg, local, m, grouped);
       j = atomicAdd(&s_next, 1u);
     }
     j = __shfl_sync(0xffffffffu, j, 0);
@@ -847,7 +881,7 @@ struct TmaLayout {
 // The CTA owns rows b, b + grid, ... (see k_reduce_ldg); its first NW * depth rows start the
 // stages, the rest are handed out through a counter behind the barriers in shared memory, since
 // rows now cost anything from a head to a full read.
-template <int NW>
+template <int NW, bool kGroups = false>
 __global__ void __launch_bounds__(NW * 32) k_reduce_tma(ReduceParams p, TmaLayout L) {
   extern __shared__ __align__(128) unsigned char smem[];
   const int lane = threadIdx.x & 31;
@@ -918,13 +952,13 @@ __global__ void __launch_bounds__(NW * 32) k_reduce_tma(ReduceParams p, TmaLayou
     uint32_t seg, local;
     (void)row_ptr(p, blockIdx.x + j * gridDim.x, seg, local);
     const bool is_power = seg ? p.seg[1].is_power != 0 : p.seg[0].is_power != 0;
-    if (e0 + n < p.T && !(stop && settles(m, is_power, p.thr))) {
+    if (e0 + n < p.T && !(stop && settles(m, is_power, p.thr) && !(kGroups && row_grouped(p, seg, local)))) {
       issue(s, j, ++c);
     } else {
       uint32_t next = 0;
       if (lane == 0) {
         if (!scratch_ok) wait_scratch_free(p), scratch_ok = true;
-        publish_row(p, seg, local, m);
+        publish_row(p, seg, local, m, kGroups && row_grouped(p, seg, local));
         next = atomicAdd(next_row, 1u);
       }
       j = min(__shfl_sync(0xffffffffu, next, 0), n_rows), c = 0, m = nan_f();

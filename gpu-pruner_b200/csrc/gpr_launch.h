@@ -120,6 +120,14 @@ inline uint32_t fold_grid(const LaunchKnobs& k, uint32_t P) {
   return std::max<uint32_t>(1u, std::min<uint32_t>((W + 4u * warps - 1u) / (4u * warps), (uint32_t)k.sm_count));
 }
 
+// k_group_rows / k_group_sum (gpr_groups.cuh, only with a group table): CTAs of kGroupBlock threads, one warp per pod
+// and round, at most 8 CTAs per SM; both kernels loop over the pods (k_group_sum over the listed ones).
+constexpr uint32_t kGroupBlock = 256;
+inline uint32_t group_grid(const LaunchKnobs& k, uint32_t P) {
+  const uint64_t ctas = ((uint64_t)P + kGroupBlock / 32u - 1u) / (kGroupBlock / 32u);
+  return (uint32_t)std::max<uint64_t>(1u, std::min<uint64_t>(ctas, (uint64_t)k.sm_count * 8u));
+}
+
 // rounds of fold_words' outer loop for the first warp of the fold grid
 inline uint32_t fold_rounds(const LaunchKnobs& k, uint32_t P) {
   const uint32_t W = (uint32_t)(((uint64_t)P + 31u) / 32u);

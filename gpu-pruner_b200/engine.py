@@ -42,6 +42,7 @@ class Decision:
     n_decisions: int
     kernel_ms: float
     veto_bits: Optional[np.ndarray] = None   # uint32[ceil(P/32)]: pods vetoed by the power clause (this rank's pods)
+    idle_slots: Optional[np.ndarray] = None  # uint32[P, ceil(G/32)]: slots that start an idle element
 
     def pods(self, bits: Optional[np.ndarray] = None) -> np.ndarray:
         """Indices of set bits (the idle-pod set), ascending."""
@@ -132,8 +133,9 @@ class IdleEngine:
 
     # ---- hot path ---------------------------------------------------------------------------
     def _window(self, util, power, eligible, created_ts, cutoff_ts, P, G, T, row_stride,
-                power_threshold, mem_kind, util_format: int = ffi.GPR_FMT_F32) -> ffi.gpr_window:
+                power_threshold, mem_kind, util_format: int = ffi.GPR_FMT_F32, groups=None) -> ffi.gpr_window:
         w = ffi.gpr_window()
+        w.groups = _ptr(groups)
         w.util_format = util_format
         w.struct_size = C.sizeof(ffi.gpr_window)
         w.mem_kind = mem_kind
@@ -149,9 +151,11 @@ class IdleEngine:
                eligible: Optional[np.ndarray] = None, created_ts: Optional[np.ndarray] = None,
                cutoff_ts: int = 0, power_threshold: Optional[float] = 0.0,
                want_candidates: bool = True, want_series_max: bool = False,
-               world: int = 1, want_veto: bool = False) -> Decision:
+               world: int = 1, want_veto: bool = False, groups: Optional[np.ndarray] = None,
+               want_idle_slots: bool = False) -> Decision:
         """Blocking decision over a HOST window ``util[P, G, T]`` (float32, NaN = no sample; or
-        uint8 in the biased byte format GPR_FMT_U8B, see :func:`to_biased_u8`)."""
+        uint8 in the biased byte format GPR_FMT_U8B, see :func:`to_biased_u8`).  ``groups``: the
+        ``sum by`` group table ``uint32[P, G]`` (include/gpr.h, gpr_window.groups)."""
         fmt = ffi.GPR_FMT_U8B if getattr(util, "dtype", None) == np.uint8 else ffi.GPR_FMT_F32
         util = np.ascontiguousarray(util, dtype=np.uint8 if fmt else np.float32)
         if util.ndim != 3:
@@ -165,9 +169,14 @@ class IdleEngine:
             eligible = np.ascontiguousarray(eligible, dtype=np.uint8)
         if created_ts is not None:
             created_ts = np.ascontiguousarray(created_ts, dtype=np.int64)
+        if groups is not None:
+            groups = np.ascontiguousarray(groups, dtype=np.uint32)
+            if groups.shape != (P, G):
+                raise ValueError("groups must be [pods, gpus]")
         w = self._window(util, power, eligible, created_ts, cutoff_ts, P, G, T, 0,
-                         power_threshold, ffi.GPR_MEM_HOST, fmt)
+                         power_threshold, ffi.GPR_MEM_HOST, fmt, groups)
         W = (P + 31) // 32 * world
+        islots = np.zeros((max(P, 1), (G + 31) // 32), dtype=np.uint32) if want_idle_slots else None
         dbits = np.zeros(max(W, 1), dtype=np.uint32)
         cbits = np.zeros(max(W, 1), dtype=np.uint32) if want_candidates else None
         smax = np.zeros((P, G), dtype=np.float32) if want_series_max else None
@@ -177,10 +186,12 @@ class IdleEngine:
         r.out_mem_kind = ffi.GPR_MEM_HOST
         r.decision_bits, r.candidate_bits, r.series_max = _ptr(dbits), _ptr(cbits), _ptr(smax)
         r.veto_bits = _ptr(vbits)
+        r.idle_slots = _ptr(islots)
         self._check(self._lib.gpr_decide(self._h, C.byref(w), C.byref(r)))
         d = Decision(P, dbits[:W], None if cbits is None else cbits[:W], smax, r.n_series,
                      r.n_candidates, r.n_decisions, r.kernel_ms)
         d.veto_bits = None if vbits is None else vbits[:(P + 31) // 32]
+        d.idle_slots = None if islots is None else islots[:P]
         return d
 
     def decide_ptr(self, util, P: int, G: int, T: int, decision_bits, *, power=None, eligible=None,
@@ -188,17 +199,20 @@ class IdleEngine:
                    candidate_bits=None, series_max=None, veto_bits=None, row_stride: int = 0,
                    in_kind: int = ffi.GPR_MEM_DEVICE, out_kind: int = ffi.GPR_MEM_DEVICE,
                    blocking: bool = True, resident: bool = False,
-                   util_format: int = ffi.GPR_FMT_F32) -> ffi.gpr_result:
+                   util_format: int = ffi.GPR_FMT_F32, groups=None, idle_slots=None) -> ffi.gpr_result:
         """Raw-pointer form (device tensors, pinned host buffers).  With ``blocking=False`` the
-        call only enqueues; counters in the returned struct are valid after :meth:`sync`."""
+        call only enqueues; counters in the returned struct are valid after :meth:`sync`.
+        ``groups`` (where ``in_kind`` says) and ``idle_slots`` (where ``out_kind`` says): see
+        include/gpr.h; ``resident=True`` is gpr_decide_resident."""
         w = self._window(util, power, eligible, created_ts, cutoff_ts, P, G, T, row_stride,
-                         power_threshold, in_kind, util_format)
+                         power_threshold, in_kind, util_format, groups)
         r = ffi.gpr_result()
         r.struct_size = C.sizeof(ffi.gpr_result)
         r.out_mem_kind = out_kind
         r.decision_bits, r.candidate_bits, r.series_max = (_ptr(decision_bits), _ptr(candidate_bits),
                                                            _ptr(series_max))
         r.veto_bits = _ptr(veto_bits)
+        r.idle_slots = _ptr(idle_slots)
         if resident:
             self._check(self._lib.gpr_decide_resident(self._h, C.byref(w), C.byref(r)))
         elif blocking:
@@ -218,7 +232,7 @@ class IdleEngine:
             w = self._window(kw["util"], kw.get("power"), kw.get("eligible"), kw.get("created_ts"),
                              kw.get("cutoff_ts", 0), kw["P"], kw["G"], kw["T"], kw.get("row_stride", 0),
                              kw.get("power_threshold", 0.0), kw.get("in_kind", ffi.GPR_MEM_DEVICE),
-                             kw.get("util_format", ffi.GPR_FMT_F32))
+                             kw.get("util_format", ffi.GPR_FMT_F32), kw.get("groups"))
             C.memmove(C.byref(wins, i * C.sizeof(ffi.gpr_window)), C.byref(w), C.sizeof(ffi.gpr_window))
             r = ress[i]
             r.struct_size = C.sizeof(ffi.gpr_result)
@@ -226,6 +240,8 @@ class IdleEngine:
             r.decision_bits = _ptr(kw["decision_bits"])
             r.candidate_bits = _ptr(kw.get("candidate_bits"))
             r.series_max = _ptr(kw.get("series_max"))
+            r.veto_bits = _ptr(kw.get("veto_bits"))
+            r.idle_slots = _ptr(kw.get("idle_slots"))
         return wins, ress, calls   # `calls` keeps the tensors alive
 
     def decide_batch_async(self, batch, n: Optional[int] = None):

@@ -20,6 +20,7 @@ GPR_KERNEL_AUTO, GPR_KERNEL_LDG, GPR_KERNEL_TMA = 0, 1, 2
 GPR_FMT_F32, GPR_FMT_U8B = 0, 1
 GPR_F_POWER_PLANE = 0x1
 GPR_F_BLOCK_INDEX = 0x2
+GPR_GROUP_UTIL = 0x100
 GPR_UNIQUE_ID_BYTES = 128
 GPR_P2P_HANDLE_BYTES = 64
 
@@ -42,6 +43,7 @@ class gpr_window(C.Structure):
         ("n_pods", C.c_uint32), ("n_gpus", C.c_uint32), ("n_samples", C.c_uint32),
         ("util_format", C.c_uint32),
         ("row_stride", C.c_uint64), ("power_threshold", C.c_double),
+        ("groups", C.c_void_p),
     ]
 
 
@@ -52,6 +54,7 @@ class gpr_result(C.Structure):
         ("veto_bits", C.c_void_p),
         ("n_series", C.c_uint64), ("n_candidates", C.c_uint64), ("n_decisions", C.c_uint64),
         ("kernel_ms", C.c_double),
+        ("idle_slots", C.c_void_p),
     ]
 
 

@@ -192,6 +192,14 @@ GPH_API int gph_group_values(const float* series_max, double* out) {
   return 0;
 }
 
+// the engine's group table (gpr_window.groups) of the last window, for `pods` pods (>= P: head-room rows lead
+// themselves): pods * G entries
+GPH_API int gph_group_table(unsigned pods, unsigned* out) {
+  const std::vector<uint32_t> t = gph::group_table(g_last_window, pods);
+  std::copy(t.begin(), t.end(), out);
+  return 0;
+}
+
 // owner walk over a fixture directory: pod_meta_json = the pod's .metadata.  JSON out:
 // {"kind":..,"name":..,"namespace":..,"uid":..,"apiVersion":..,"calls":n} or {"error":..}
 GPH_API int gph_find_root(const char* fixture_dir, const char* pod_meta_json, char* out, int cap) {

@@ -206,6 +206,7 @@ TickResult Controller::run_query_and_scale(const Window& w) {
   const uint32_t W = (P + 31) / 32;
   std::vector<uint32_t> dbits(std::max<uint32_t>(W, 1), 0), cbits(std::max<uint32_t>(W, 1), 0);
   std::vector<float> smax((size_t)P * G + 1, 0.f);
+  std::vector<uint32_t> idle_slots;   // the engine's, when it resolved the `sum by` groups itself
 
   // lookback = duration + grace (main.rs:413-414); `now` once per tick
   const int64_t now_ns = args_.now_override ? args_.now_override * 1000000000ll : clock_.now_ns();
@@ -267,13 +268,18 @@ TickResult Controller::run_query_and_scale(const Window& w) {
       out.error = "Failed to run query! " + (engine_ ? err : std::string("no idle engine"));
       return out;
     }
-    if (v.decision_bits.size() < W || v.candidate_bits.size() < W || v.series_max.size() < (size_t)P * G) {
+    const size_t MW = (G + 31) / 32;
+    if (v.decision_bits.size() < W || v.candidate_bits.size() < W ||
+        (v.groups_resolved ? v.idle_slots.size() < (size_t)P * MW : v.series_max.size() < (size_t)P * G)) {
       out.error = "Failed to run query! idle engine returned a short result";
       return out;
     }
     // pods with several series in one `sum by` group: the element is the SUM of the members' maxima
-    // (query.promql.j2:9,21); re-derived on the host from the per-series maxima, rare
-    if (v.veto_bits.size() >= W || !rq.power_on) {
+    // (query.promql.j2:9,21); the engine does that itself given the group table, otherwise it is re-derived here
+    // from the per-series maxima
+    if (v.groups_resolved) {
+      idle_slots = std::move(v.idle_slots);
+    } else if (v.veto_bits.size() >= W || !rq.power_on) {
       const GroupFixup fx = resolve_sum_by_groups(w, v.series_max.data(), v.veto_bits.size() >= W ? v.veto_bits.data() : nullptr,
                                                   rq.eligible, rq.created_ts, rq.cutoff_ts, v.candidate_bits.data(),
                                                   v.decision_bits.data(), &v.n_series, &v.n_candidates, &v.n_decisions);
@@ -289,7 +295,7 @@ TickResult Controller::run_query_and_scale(const Window& w) {
     }
     std::copy(v.decision_bits.begin(), v.decision_bits.begin() + W, dbits.begin());
     std::copy(v.candidate_bits.begin(), v.candidate_bits.begin() + W, cbits.begin());
-    std::copy(v.series_max.begin(), v.series_max.begin() + (size_t)P * G, smax.begin());
+    if (!v.groups_resolved) std::copy(v.series_max.begin(), v.series_max.begin() + (size_t)P * G, smax.begin());
     out.qr.num_pods = (size_t)v.n_series;
     out.kernel_ms = v.kernel_ms;
     out.n_candidates = v.n_candidates;
@@ -302,6 +308,19 @@ TickResult Controller::run_query_and_scale(const Window& w) {
     const PodEntry& pe = w.pods[p];
     PodMetricData pmd;
     pmd.name = pe.name, pmd.ns = pe.ns;
+    if (!idle_slots.empty()) {
+      // the first slot that starts an idle element; its value is 0 (a cancelling round-to-nearest sum is +0.0)
+      const size_t MW = (G + 31) / 32;
+      for (uint32_t g = 0; g < pe.slots.size(); ++g) {
+        if (!(idle_slots[(size_t)p * MW + (g >> 5)] >> (g & 31) & 1u)) continue;
+        const GpuSlot& s = pe.slots[g];
+        pmd.container = s.container, pmd.node_type = s.node_type, pmd.gpu_model = s.model;
+        pmd.value = 0.0;
+        break;
+      }
+      out.unique_pods.push_back(pmd);
+      continue;
+    }
     for (uint32_t g = 0; g < pe.slots.size(); ++g) {
       if (pe.slots[g].group != g) continue;              // elements are `sum by` groups (j2:9)
       const double value = group_value(w, smax.data(), p, g);

@@ -71,7 +71,11 @@ struct VerdictRequest {
 struct Verdict {
   std::vector<uint32_t> decision_bits, candidate_bits;   // ceil(P/32) words
   std::vector<uint32_t> veto_bits;                       // ceil(P/32) words or empty: pods vetoed by the power clause
-  std::vector<float> series_max;                         // [P*G]
+  std::vector<float> series_max;                         // [P*G], or empty when groups_resolved
+  // groups_resolved: the engine decided on `sum by` groups itself (gpr_window.groups), so the bits and counts are
+  // PromQL's already; idle_slots [P][ceil(G/32)] then says which slots start an idle element (gpr_result.idle_slots)
+  bool groups_resolved = false;
+  std::vector<uint32_t> idle_slots;
   uint64_t n_series = 0, n_candidates = 0, n_decisions = 0;
   double kernel_ms = 0;
 };

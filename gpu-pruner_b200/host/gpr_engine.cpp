@@ -26,6 +26,7 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
     if (ctx_) {
       if (d_elig_) gpr_device_free(ctx_, d_elig_);
       if (d_created_) gpr_device_free(ctx_, d_created_);
+      if (d_table_) gpr_device_free(ctx_, d_table_);
       gpr_destroy(ctx_);
     }
   }
@@ -40,8 +41,11 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
     if (on_device ? !ensure_ctx(rq.gpu_device, error) : !ensure(w, rq.power_on, rq.gpu_device, error)) return false;
     const uint32_t W = (w.P + 31) / 32;
     out->decision_bits.assign(W, 0), out->candidate_bits.assign(W, 0);
-    out->series_max.assign((size_t)w.P * w.G, 0.f);
-    out->veto_bits.assign(W, 0);
+    // the engine resolves `sum by` groups itself and says which slots start idle elements: no per-series maxima
+    // (the reduce stops reading a row once its flag is settled), no veto bitmap
+    out->idle_slots.assign((size_t)w.P * ((w.G + 31) / 32), 0u);
+    out->groups_resolved = true;
+    const std::vector<uint32_t> table = has_groups(w) ? group_table(w, w.P) : std::vector<uint32_t>();
     gpr_window win;
     memset(&win, 0, sizeof win);
     win.struct_size = sizeof win;
@@ -53,13 +57,14 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
       win.mem_kind = GPR_MEM_DEVICE;
       win.util = w.d_util;
       win.power = rq.power_on ? w.d_power : nullptr;
-      if (!upload_gates(rq, w.P, &win, error)) return false;
+      if (!upload_gates(rq, w.P, &win, error) || !upload_table(table, &win, error)) return false;
     } else {
       win.mem_kind = GPR_MEM_HOST;
       win.util = w.util.data();
       win.power = rq.power_on ? w.power.data() : nullptr;
       win.eligible = rq.eligible;
       win.created_ts = rq.created_ts;
+      win.groups = table.empty() ? nullptr : table.data();
     }
     gpr_result res;
     memset(&res, 0, sizeof res);
@@ -67,8 +72,7 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
     res.out_mem_kind = GPR_MEM_HOST;
     res.decision_bits = out->decision_bits.data();
     res.candidate_bits = out->candidate_bits.data();
-    res.series_max = out->series_max.data();
-    res.veto_bits = out->veto_bits.data();
+    res.idle_slots = out->idle_slots.data();
     const int rc = gpr_decide(ctx_, &win, &res);
     if (rc != GPR_OK) {
       *error = "idle engine (" + std::to_string(rc) + "): " + gpr_last_error(ctx_);
@@ -87,9 +91,9 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
       return false;
     }
     // the ring has rows for resident_pods pods; the ones beyond the pods known so far hold no sample
-    const uint32_t Pr = w.resident_pods, W = (Pr + 31) / 32;
-    std::vector<uint32_t> dbits(W, 0), cbits(W, 0), vbits(W, 0);
-    std::vector<float> smax((size_t)Pr * w.G, 0.f);
+    const uint32_t Pr = w.resident_pods, W = (Pr + 31) / 32, MW = (w.G + 31) / 32;
+    std::vector<uint32_t> dbits(W, 0), cbits(W, 0), islots((size_t)Pr * MW, 0u);
+    const std::vector<uint32_t> table = has_groups(w) ? group_table(w, Pr) : std::vector<uint32_t>();
     std::vector<uint8_t> elig(Pr, 0);
     std::vector<int64_t> created(Pr, std::numeric_limits<int64_t>::max());
     for (uint32_t p = 0; p < w.P; ++p) {
@@ -104,12 +108,12 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
     win.cutoff_ts = rq.cutoff_ts;
     win.eligible = elig.data();
     win.created_ts = rq.created_ts ? created.data() : nullptr;
+    win.groups = table.empty() ? nullptr : table.data();
     gpr_result res;
     memset(&res, 0, sizeof res);
     res.struct_size = sizeof res;
     res.out_mem_kind = GPR_MEM_HOST;
-    res.decision_bits = dbits.data(), res.candidate_bits = cbits.data(), res.veto_bits = vbits.data();
-    res.series_max = smax.data();
+    res.decision_bits = dbits.data(), res.candidate_bits = cbits.data(), res.idle_slots = islots.data();
     const int rc = gpr_decide_resident(ctx_, &win, &res);
     if (rc != GPR_OK) {
       *error = "idle engine (" + std::to_string(rc) + "): " + gpr_last_error(ctx_);
@@ -118,8 +122,8 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
     const uint32_t Wp = (w.P + 31) / 32;
     out->decision_bits.assign(dbits.begin(), dbits.begin() + Wp);
     out->candidate_bits.assign(cbits.begin(), cbits.begin() + Wp);
-    out->veto_bits.assign(vbits.begin(), vbits.begin() + Wp);
-    out->series_max.assign(smax.begin(), smax.begin() + (size_t)w.P * w.G);
+    out->idle_slots.assign(islots.begin(), islots.begin() + (size_t)w.P * MW);
+    out->groups_resolved = true;
     out->n_series = res.n_series, out->n_candidates = res.n_candidates, out->n_decisions = res.n_decisions;
     out->kernel_ms = res.kernel_ms;
     return true;
@@ -226,6 +230,32 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
   }
 
   // ---- context ------------------------------------------------------------------------------------------
+  static bool has_groups(const Window& w) {
+    for (const PodEntry& pe : w.pods)
+      if (pe.has_groups) return true;
+    return false;
+  }
+  // the group table of a device window lives on the device too (gpr_window.groups follows mem_kind)
+  bool upload_table(const std::vector<uint32_t>& table, gpr_window* win, std::string* error) {
+    if (table.empty()) return true;
+    const size_t bytes = table.size() * sizeof(uint32_t);
+    if (bytes > table_cap_) {
+      if (d_table_) gpr_device_free(ctx_, d_table_), d_table_ = nullptr;
+      table_cap_ = 0;
+      if (gpr_device_alloc(ctx_, bytes + bytes / 4 + 256, &d_table_) != GPR_OK) {
+        *error = std::string("idle engine: group table buffer: ") + gpr_last_error(ctx_);
+        return false;
+      }
+      table_cap_ = bytes + bytes / 4 + 256;
+    }
+    if (gpr_memcpy(ctx_, d_table_, table.data(), bytes, GPR_MEM_DEVICE, GPR_MEM_HOST) != GPR_OK) {
+      *error = std::string("idle engine: group table upload: ") + gpr_last_error(ctx_);
+      return false;
+    }
+    win->groups = static_cast<const uint32_t*>(d_table_);
+    return true;
+  }
+
   bool upload_gates(const VerdictRequest& rq, uint32_t P, gpr_window* win, std::string* error) {
     if (P > gate_cap_) {
       if (d_elig_) gpr_device_free(ctx_, d_elig_), d_elig_ = nullptr;
@@ -271,7 +301,8 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
     session_.reset();  // its resident window dies with the context
     if (d_elig_) gpr_device_free(ctx_, d_elig_), d_elig_ = nullptr;
     if (d_created_) gpr_device_free(ctx_, d_created_), d_created_ = nullptr;
-    gate_cap_ = 0;
+    if (d_table_) gpr_device_free(ctx_, d_table_), d_table_ = nullptr;
+    gate_cap_ = 0, table_cap_ = 0;
     gpr_destroy(ctx_), ctx_ = nullptr;
   }
   bool create(uint32_t max_pods, uint32_t max_gpus, uint32_t max_samples, bool need_power, int device,
@@ -300,6 +331,8 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
   void* d_elig_ = nullptr;
   void* d_created_ = nullptr;
   size_t gate_cap_ = 0;
+  void* d_table_ = nullptr;
+  size_t table_cap_ = 0;
 };
 
 }  // namespace

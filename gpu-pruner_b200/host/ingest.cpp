@@ -4,6 +4,7 @@
 #include <unordered_map>
 
 #include "ingest_internal.hpp"
+#include "../../include/gpr.h"
 
 namespace gph {
 
@@ -302,6 +303,20 @@ double group_value(const Window& w, const float* series_max, uint32_t p, uint32_
     k.add(pe.slots[g].from_prof ? (double)m : (double)m / 100.0);
   }
   return k.any ? k.value() : std::numeric_limits<double>::quiet_NaN();
+}
+
+std::vector<uint32_t> group_table(const Window& w, uint32_t pods) {
+  std::vector<uint32_t> t((size_t)pods * w.G);
+  for (uint32_t p = 0; p < pods; ++p)
+    for (uint32_t g = 0; g < w.G; ++g) {
+      uint32_t e = g;
+      if (p < w.P && g < w.pods[p].slots.size()) {
+        const GpuSlot& s = w.pods[p].slots[g];
+        e = s.group | (s.from_prof ? 0u : (uint32_t)GPR_GROUP_UTIL);
+      }
+      t[(size_t)p * w.G + g] = e;
+    }
+  return t;
 }
 
 GroupFixup resolve_sum_by_groups(const Window& w, const float* series_max, const uint32_t* veto_bits,

@@ -146,5 +146,9 @@ GroupFixup resolve_sum_by_groups(const Window& w, const float* series_max, const
 // value of the element (group) that slot `slot` of pod `p` starts, from the per-series maxima: what
 // Prometheus reports for it (NaN = no element)
 double group_value(const Window& w, const float* series_max, uint32_t p, uint32_t slot);
+// The same groups as the engine's table (gpr_window.groups, include/gpr.h): [pods][G] entries, bits 0-7 the slot of the
+// group's first member, GPR_GROUP_UTIL for a GPU_UTIL member.  Slots beyond a pod's series and pods beyond w.P (the
+// head-room rows of a resident ring) lead themselves.  The one place on the host that knows the encoding.
+std::vector<uint32_t> group_table(const Window& w, uint32_t pods);
 
 }  // namespace gph

@@ -142,6 +142,24 @@ typedef struct gpr_config {
  *   created_ts[p]   i64 or NULL: pod creation time in caller-chosen ticks; the pod is skipped
  *                   iff created_ts[p] >= cutoff_ts   (main.rs:494,508-510, cutoff = now -
  *                   (duration*60 + grace_period)).  INT64_MAX = "no creationTimestamp".
+ *   groups[p][g]    u32 or NULL (follows mem_kind like the gates): the `sum by (Hostname, container,
+ *                   pod, namespace, gpu, modelName)` groups of the query (query.promql.j2:9,21), for
+ *                   callers whose window keeps several series of one group in separate rows.
+ *                   Bits 0-7: slot of the group's first member (its leader), <= g; a leader's own
+ *                   entry leads itself.  GPR_GROUP_UTIL: the row is a DCGM_FI_DEV_GPU_UTIL series,
+ *                   divided by 100 before the sum (j2:20); without it the row is summed as it is
+ *                   (DCGM_FI_PROF_GR_ENGINE_ACTIVE).  Any other bit, a leader > g or a leader whose
+ *                   entry is not its own is GPR_E_INVALID (a host table before anything is enqueued,
+ *                   a device table at gpr_sync / the blocking call's return).
+ *                   With a table an element is a group, not a row: its value is Prometheus' sum
+ *                   (Neumaier-compensated float64, in slot order) of the window maxima of its
+ *                   members that have a sample, NaN if none has; the element is idle iff value == 0.
+ *                   candidate = some idle element && !veto; n_series counts idle elements.  A row of
+ *                   a group of two or more is read whole (no early exit).  series_max and veto_bits
+ *                   keep their per-row meaning; the power plane is never grouped (`unless on` needs
+ *                   no grouping).  NULL: every row is its own element, as before.
+ *   struct_size     sizeof(gpr_window), or offsetof(gpr_window, groups) for a caller built before
+ *                   `groups` existed (no table).
  */
 typedef struct gpr_window {
   uint32_t struct_size;
@@ -157,7 +175,10 @@ typedef struct gpr_window {
   uint32_t util_format;    /* GPR_FMT_*; ignored by gpr_decide_resident (the ring is f32)   */
   uint64_t row_stride;
   double power_threshold;
+  const uint32_t *groups;
 } gpr_window;
+
+#define GPR_GROUP_UTIL 0x100u /* gpr_window.groups: a GPU_UTIL member, summed as max / 100 (bits 0-7: leader) */
 
 /*
  * Result.  Bitmaps are packed little-endian within a word: pod p is bit (p & 31) of word
@@ -175,9 +196,15 @@ typedef struct gpr_window {
  *                   power series at or above the threshold (the `unless on (pod, namespace)` clause,
  *                   query.promql.j2:36-44).  With series_max it lets a caller re-derive a pod's verdict
  *                   (exact `sum by` of duplicate series, gpu-pruner_b200/host/ingest.cpp).
+ *   idle_slots      optional, n_pods * ceil(n_gpus/32) words, THIS rank's pods only: bit g of pod p's
+ *                   words is set iff slot g starts an element whose value is == 0 — without a group
+ *                   table iff row g's window max == 0; with one iff g leads a group whose sum is == 0
+ *                   (members are never set).  Veto and gates do not touch it.  The first set bit of a
+ *                   candidate pod is the element the reference reports (main.rs:430-435, value 0).
  *   out_mem_kind    where the buffers above live.
- *   n_series        number of idle series in non-vetoed pods = QueryResponse.num_pods
- *                   (main.rs:418; a series count despite the name).
+ *   n_series        number of idle elements (series, or groups with gpr_window.groups) in non-vetoed
+ *                   pods = QueryResponse.num_pods (main.rs:418; a series count despite the name).
+ *   struct_size     sizeof(gpr_result), or offsetof(gpr_result, idle_slots) (no idle_slots).
  *   n_candidates / n_decisions   popcounts of the two bitmaps (this rank's pods).
  *   kernel_ms       device time of the decision kernel(s) for this call (CUDA events);
  *                   0 from the _async entry point.
@@ -193,6 +220,7 @@ typedef struct gpr_result {
   uint64_t n_candidates;
   uint64_t n_decisions;
   double kernel_ms;
+  uint32_t *idle_slots;
 } gpr_result;
 
 /* ---- lifecycle ----------------------------------------------------------------------- */
