@@ -27,6 +27,7 @@
 
 #include "gpr_kernels.cuh"
 #include "gpr_groups.cuh"
+#include "gpr_probe.cuh"
 #include "gpr_ring.cuh"
 #include "gpr_synth.cuh"
 #include "gpr_text_kernels.cuh"
@@ -36,6 +37,7 @@ namespace {
 using gpr::kLdgUnroll;
 using gpr::kLdgWarps;
 using gpr::kTmaSmemBudget;
+using gpr::kProbeSmemBudget;
 constexpr int kSlots = 256;      // outstanding async results
 constexpr int kMaxChunkEvents = 64;
 constexpr int kExchangeDepth = 4;  // exchange buffer sets of the fused multi-GPU path = 2 x scratch sets
@@ -334,11 +336,16 @@ cudaError_t launch_tma(gpr_ctx* ctx, const gpr::ReduceParams& rp, const gpr::Red
 template <bool kGroups>
 int launch_reduce_as(gpr_ctx* ctx, gpr::ReduceParams& rp, bool tma_ok, bool pdl) {
   if (rp.total_rows == 0) return GPR_OK;
-  // AUTO = the TMA pipeline (measured winner on H100 at C2 and C3, DESIGN.md §4.3); rows that are
-  // not 16-byte aligned or have T % 4 != 0 cannot be bulk-copied and take the LDG kernel
-  const gpr::ReducePlan plan = gpr::plan_reduce(launch_knobs(ctx), rp.T, rp.total_rows, tma_ok, rp.util_u8 != 0);
+  // AUTO = the probe kernel when every row may stop early, else the TMA pipeline (DESIGN.md §4.3); rows
+  // that are not 16-byte aligned or have T % 4 != 0 cannot be bulk-copied and take the LDG kernel.
+  // Rows may stop unless the call asks for series_max (the host-side form of rows_may_stop) or has a group table.
+  const bool may_stop = !kGroups && rp.seg[0].smax == nullptr && rp.seg[1].smax == nullptr;
+  const gpr::ReducePlan plan =
+      gpr::plan_reduce(launch_knobs(ctx), rp.T, rp.total_rows, tma_ok, rp.util_u8 != 0, may_stop);
   cudaError_t e;
-  if (plan.kernel == gpr::kReduceU8) {
+  if (plan.kernel == gpr::kReduceProbe) {
+    e = launch_ex(gpr::k_reduce_probe<gpr::kProbeWarps>, plan.grid, plan.block, plan.smem, ctx->stream, pdl, rp, plan.L);
+  } else if (plan.kernel == gpr::kReduceU8) {
     e = launch_ex(gpr::k_reduce_u8<kLdgWarps, gpr::kU8Unroll, kGroups>, plan.grid, plan.block, 0, ctx->stream, pdl, rp);
   } else if (plan.kernel == gpr::kReduceTma) {
     const int nw = ctx->tma_warps;
@@ -1119,6 +1126,8 @@ int gpr_create(const gpr_config* cfg, gpr_ctx** out) {
                             (int)kTmaSmemBudget));
     CU(cudaFuncSetAttribute(gpr::k_reduce_tma<32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             (int)kTmaSmemBudget));
+    CU(cudaFuncSetAttribute(gpr::k_reduce_probe<gpr::kProbeWarps>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)kProbeSmemBudget));
     // (the instantiations for calls with a `sum by` group table)
     CU(cudaFuncSetAttribute(gpr::k_reduce_tma<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             (int)kTmaSmemBudget));

@@ -24,6 +24,16 @@ constexpr size_t kTmaSmemBudget = 208 * 1024;
 // sample, so the head is all that is read of them; a row the head does not settle is read on in chunk_elems chunks.
 constexpr uint32_t kTmaHeadElems = 128;
 constexpr uint32_t kTmaMaxDepth = 32;   // k_reduce_tma keeps the row of stage s in lane s
+// k_reduce_probe (gpr_probe.cuh), the AUTO kernel of calls whose rows may stop: a 32-sample head, then 512-sample
+// chunks (DESIGN.md §4.1).  Most busy rows settle in their first samples and pay 128 B; a row that settles late pays
+// at most one 2 KB chunk past its first settling sample.  One CTA of kProbeWarps warps per SM on the full budget:
+// 3 stages per warp at T >= 512, 96 rows in flight.  A warp serves its landed stages one after another, so the rows
+// are spread over as many warps as a CTA holds; 16 warps of 6 stages were 8 % slower at C2 (DESIGN.md §4.3).
+constexpr uint32_t kProbeHeadElems = 32;
+constexpr uint32_t kProbeChunkElems = 512;
+constexpr int kProbeCtasPerSm = 1;
+constexpr int kProbeWarps = 32;
+constexpr size_t kProbeSmemBudget = kTmaSmemBudget;
 
 // (the same definition, under the same guard, is in gpr_kernels.cuh's namespace body, which must also compile alone)
 #ifndef GPR_TMA_LAYOUT_DEFINED
@@ -49,7 +59,7 @@ struct LaunchKnobs {
   int fold_threads = 256;     // 64, 128 or 256
 };
 
-enum ReduceKernel { kReduceLdg = 1, kReduceTma = 2, kReduceU8 = 3 };
+enum ReduceKernel { kReduceLdg = 1, kReduceTma = 2, kReduceU8 = 3, kReduceProbe = 4 };
 // why a TMA request runs the LDG kernel instead
 enum TmaFallback { kNoFallback = 0, kFallbackAlignment = 1, kFallbackSmem = 2 };
 
@@ -58,7 +68,7 @@ struct ReducePlan {
   int fallback;      // TmaFallback
   uint32_t grid, block;
   size_t smem;       // dynamic shared memory (TMA only)
-  TmaLayout L;       // TMA only
+  TmaLayout L;       // TMA and probe only
 };
 
 // Rows are cut into n_chunks nearly equal chunks of at most tma_chunk_bytes, each a multiple of 4 elements
@@ -85,10 +95,38 @@ inline size_t tma_smem_bytes(const TmaLayout& L, int nw) {
   return (size_t)nw * L.depth * L.stage_bytes + (size_t)nw * L.depth * sizeof(uint64_t) + sizeof(uint64_t);
 }
 
+// k_reduce_probe's ring: stages of one chunk (a window shorter than a chunk gets stages of its own length), as many
+// per warp as kProbeSmemBudget holds, at most kTmaMaxDepth.  The tma knobs do not apply.
+// n_chunks = copies of a row read to its end.
+inline TmaLayout probe_layout(uint32_t T, int nw) {
+  TmaLayout L;
+  L.chunk_elems = std::min<uint32_t>(kProbeChunkElems, std::max<uint32_t>((T + 3u) & ~3u, 4u));
+  L.head_elems = std::min<uint32_t>(kProbeHeadElems, L.chunk_elems);
+  L.n_chunks = 1u + (T > L.head_elems ? (T - L.head_elems + L.chunk_elems - 1u) / L.chunk_elems : 0u);
+  L.stage_bytes = (L.chunk_elems * 4u + 127u) & ~127u;
+  // (each stage also has its 8-byte barrier, and the CTA one row counter: short stages make the barriers count)
+  const uint32_t d = (uint32_t)((kProbeSmemBudget - 8) / (((size_t)L.stage_bytes + 8) * nw));
+  L.depth = std::max<uint32_t>(std::min<uint32_t>(d, kTmaMaxDepth), 1u);
+  return L;
+}
+
 // The reduce launch for `total_rows` rows of T samples.  tma_ok: every row base is 16-byte aligned and T % 4 == 0
-// (what a bulk copy needs); util_u8: the util plane is in GPR_FMT_U8B.  AUTO means TMA (DESIGN.md §4.3).
-inline ReducePlan plan_reduce(const LaunchKnobs& k, uint32_t T, uint32_t total_rows, bool tma_ok, bool util_u8) {
+// (what a bulk copy needs); util_u8: the util plane is in GPR_FMT_U8B; may_stop: every row may stop at its first
+// settling sample (no series_max target and no group table, so no row is read whole for its max).  AUTO means the
+// probe kernel when rows may stop and the bulk copies and the f32 util plane allow it, else TMA (DESIGN.md §4.3).
+inline ReducePlan plan_reduce(const LaunchKnobs& k, uint32_t T, uint32_t total_rows, bool tma_ok, bool util_u8,
+                              bool may_stop = false) {
   ReducePlan r = {};
+  if (k.variant == GPR_KERNEL_AUTO && may_stop && tma_ok && !util_u8) {
+    const int nw = kProbeWarps;
+    r.kernel = kReduceProbe;
+    r.grid = (uint32_t)std::max<uint64_t>(
+        1, std::min<uint64_t>((uint64_t)k.sm_count * kProbeCtasPerSm, ((uint64_t)total_rows + nw - 1) / nw));
+    r.block = (uint32_t)nw * 32u;
+    r.L = probe_layout(T, nw);
+    r.smem = tma_smem_bytes(r.L, nw);
+    return r;
+  }
   int variant = k.variant == GPR_KERNEL_AUTO ? GPR_KERNEL_TMA : k.variant;
   if (variant == GPR_KERNEL_TMA && !tma_ok) variant = GPR_KERNEL_LDG, r.fallback = kFallbackAlignment;
   if (variant == GPR_KERNEL_TMA && tma_smem_bytes(tma_layout(k, T, k.tma_warps), k.tma_warps) > kTmaSmemBudget)
