@@ -1,11 +1,13 @@
 """The launch geometry of gpu-pruner_b200/csrc/gpr_launch.h, queried through tests/cpp/launch_plan.cpp: which reduce
-kernel the library runs for a window on a device with given knobs, its grid and TMA ring layout, and the fold grid."""
+kernel the library runs for a window on a device with given knobs, its grid and TMA ring layout, and the fold grid.
+may_stop: the call passes no series_max target and no group table, so its rows may stop early (AUTO then runs the
+probe kernel, k_reduce_probe, when the rows can be bulk-copied and the util plane is f32)."""
 import os
 import subprocess
 from dataclasses import dataclass
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-KERNELS = {1: "ldg", 2: "tma", 3: "u8"}
+KERNELS = {1: "ldg", 2: "tma", 3: "u8", 4: "probe"}
 FALLBACKS = {0: None, 1: "alignment", 2: "smem"}
 VARIANT = {"auto": 0, "ldg": 1, "tma": 2}
 
@@ -39,6 +41,7 @@ class Plan:
     n_chunks: int
     fold_grid: int
     fold_rounds: int
+    head_elems: int
 
     def last_chunk(self, T):
         return T - (self.n_chunks - 1) * self.chunk_elems
@@ -52,9 +55,14 @@ def build(out_dir):
 
 
 def plans(exe, queries):
-    """queries: (knobs, variant, T, total_rows, tma_ok, util_u8, P) -> [Plan]"""
-    lines = [f"{k.sm_count} {VARIANT[v]} {k.tma_warps} {k.tma_chunk} {k.tma_depth} {k.ldg_ctas} {k.fold_threads} "
-             f"{T} {rows} {int(ok)} {int(u8)} {P}" for k, v, T, rows, ok, u8, P in queries]
+    """queries: (knobs, variant, T, total_rows, tma_ok, util_u8, P[, may_stop]) -> [Plan]; may_stop defaults to
+    False, the plan of a call that reads every row whole"""
+    lines = []
+    for q in queries:
+        k, v, T, rows, ok, u8, P = q[:7]
+        may_stop = q[7] if len(q) > 7 else False
+        lines.append(f"{k.sm_count} {VARIANT[v]} {k.tma_warps} {k.tma_chunk} {k.tma_depth} {k.ldg_ctas} "
+                     f"{k.fold_threads} {T} {rows} {int(ok)} {int(u8)} {P} {int(may_stop)}")
     r = subprocess.run([exe], input="\n".join(lines) + "\n", capture_output=True, text=True, check=True, timeout=60)
     out = []
     for l in r.stdout.splitlines():
@@ -64,5 +72,5 @@ def plans(exe, queries):
     return out
 
 
-def plan(exe, knobs, variant, T, total_rows, tma_ok=True, util_u8=False, P=1):
-    return plans(exe, [(knobs, variant, T, total_rows, tma_ok, util_u8, P)])[0]
+def plan(exe, knobs, variant, T, total_rows, tma_ok=True, util_u8=False, P=1, may_stop=False):
+    return plans(exe, [(knobs, variant, T, total_rows, tma_ok, util_u8, P, may_stop)])[0]

@@ -46,7 +46,7 @@ def test_boundary_and_edge_windows(kernel, oracle_np):
                             wrows[:, :T] = power.reshape(P * G, T)
                             w_dev = torch.from_numpy(wflat).to(DEV)
                             w_t = w_dev[offset:].data_ptr()
-                        bits, cbits, counts, sm, vb = _device_decide(
+                        bits, cbits, counts, sm, vb, _ = _device_decide(
                             eng, u_t[offset:].data_ptr(), P, G, T, w_t, {}, EE.THR if use_power else 0.0,
                             stride=stride, want_smax=smax, want_veto=True)
                         _check(bits, cbits, counts, exp, sm, vb if use_power else None)
@@ -108,7 +108,7 @@ def test_synthetic_windows_equal_the_c_oracle(kernel, shape, oracle_c):
             u, w, e = _synth(eng, 0x5EED0002, P, G, T, power)
             for smax in (False, True):
                 exp = _oracle_synth(oracle_c, 0x5EED0002, P, G, T, power, smax=True)
-                bits, cbits, counts, sm, vb = _device_decide(
+                bits, cbits, counts, sm, vb, _ = _device_decide(
                     eng, u, P, G, T, w, {"eligible": e.cpu().numpy()}, 150.0 if power else 0.0, want_smax=smax,
                     want_veto=power)
                 _check(bits, cbits, counts, exp, sm, vb if power else None)

@@ -5,9 +5,10 @@
   value of every knob.  Each runs test_gpu_parity's random windows, strided and misaligned rows, a host window staged
   in many chunks and a batch of unlike decisions, all against the C oracle; the geometry header
   (gpu-pruner_b200/csrc/gpr_launch.h, through tests/cpp/launch_plan.cpp) says which kernel ran, and the test asserts
-  it was the one the set is about, not a fallback.
-* Scale: device windows from gpr_synth_fill against the streaming oracle, every row checked (series_max, veto bits),
-  where the fold loops (more than 4 * (fold_threads / 32) * sm_count bitmap words).
+  it was the one the set is about, not a fallback.  The AUTO sets decide their windows twice: with series_max (every
+  row read whole, k_reduce_tma) and with idle_slots alone (rows stop early, the probe kernel), every row checked.
+* Scale: device windows from gpr_synth_fill against the streaming oracle, every row checked (series_max or
+  idle_slots, veto bits), where the fold loops (more than 4 * (fold_threads / 32) * sm_count bitmap words).
 * Limit (slow): a window of 2^31 - 32 series with a power plane, 2^32 - 64 rows in one reduce launch.
 
 Large allocations check the free device memory first and skip when it is not there: the GPU may be shared.
@@ -22,7 +23,7 @@ import pytest
 
 import geometry
 import kat
-from test_gpu_parity import SHAPES, _random_window
+from test_gpu_parity import SHAPES, _random_window, check_idle_slots
 
 pytestmark = pytest.mark.gpu
 
@@ -98,7 +99,7 @@ def _u32(t):
     return t.cpu().numpy().view(np.uint32)
 
 
-def _check(bits, cbits, counts, exp, smax=None, vbits=None):
+def _check(bits, cbits, counts, exp, smax=None, vbits=None, islots=None):
     assert np.array_equal(bits, exp["decision_bits"]), "decision bitmap differs from oracle"
     assert np.array_equal(cbits, exp["candidate_bits"]), "candidate bitmap differs from oracle"
     assert tuple(counts) == (exp["n_series"], exp["n_candidates"], exp["n_decisions"])
@@ -106,16 +107,25 @@ def _check(bits, cbits, counts, exp, smax=None, vbits=None):
         assert kat.smax_equal(smax, exp["series_max"]), "series_max differs from oracle"
     if vbits is not None:
         assert np.array_equal(vbits, exp["veto_bits"]), "veto bitmap differs from oracle"
+    if islots is not None:
+        check_idle_slots(islots, exp["series_max"])
 
 
-def _assert_intended(plan_exe, knobs, kernel, T, rows, P, tma_ok=True, util_u8=False):
-    """the geometry header's verdict for this call: the set's own kernel, with the set's own shape"""
-    p = geometry.plan(plan_exe, knobs, kernel, T, rows, tma_ok, util_u8, P)
+def _assert_intended(plan_exe, knobs, kernel, T, rows, P, tma_ok=True, util_u8=False, may_stop=False):
+    """the geometry header's verdict for this call: the set's own kernel, with the set's own shape.  may_stop: the
+    call passes no series_max (and no group table), so AUTO runs the probe kernel, whose layout ignores the tma knobs"""
+    p = geometry.plan(plan_exe, knobs, kernel, T, rows, tma_ok, util_u8, P, may_stop)
     if util_u8:
         assert p.kernel == "u8", p
     elif kernel == "ldg" or not tma_ok:
         assert p.kernel == "ldg" and p.fallback == (None if kernel == "ldg" else "alignment"), p
         assert p.grid == max(1, min(knobs.sm_count * knobs.ldg_ctas, (rows + 15) // 16)), p
+    elif kernel == "auto" and may_stop:
+        assert p.kernel == "probe" and p.fallback is None and p.block == 1024, p
+        assert p.grid == max(1, min(knobs.sm_count, (rows + 31) // 32)), p
+        base = geometry.plan(plan_exe, K(sm_count=knobs.sm_count), kernel, T, rows, tma_ok, util_u8, P, may_stop)
+        assert (p.depth, p.stage_bytes, p.chunk_elems, p.n_chunks, p.head_elems, p.smem) == \
+            (base.depth, base.stage_bytes, base.chunk_elems, base.n_chunks, base.head_elems, base.smem), (p, base)
     else:
         assert p.kernel == "tma" and p.fallback is None and p.block == 32 * knobs.tma_warps, p
         assert p.depth <= knobs.tma_depth and 4 * p.chunk_elems <= max(knobs.tma_chunk, 16), p
@@ -124,7 +134,9 @@ def _assert_intended(plan_exe, knobs, kernel, T, rows, P, tma_ok=True, util_u8=F
 
 
 def _device_decide(eng, u_t, P, G, T, w_t=None, kw=None, thr=0.0, stride=0, util_format=0, want_smax=True,
-                   want_veto=False):
+                   want_veto=False, want_slots=False):
+    """-> bits, candidate bits, counts, series_max, veto bits, idle_slots ([P, ceil(G / 32)]); the last three None
+    unless asked for"""
     kw = kw or {}
     e_t = torch.from_numpy(np.ascontiguousarray(kw["eligible"], np.uint8)).to(DEV) if "eligible" in kw else None
     c_t = torch.from_numpy(np.ascontiguousarray(kw["created_ts"], np.int64)).to(DEV) if "created_ts" in kw else None
@@ -133,13 +145,16 @@ def _device_decide(eng, u_t, P, G, T, w_t=None, kw=None, thr=0.0, stride=0, util
     cb = torch.full((W,), 0x7BADBEEF, dtype=torch.int32, device=DEV)
     vb = torch.full((W,), 0x5A5A5A5A, dtype=torch.int32, device=DEV) if want_veto else None
     sm = torch.full((max(P * G, 1),), -777.0, dtype=torch.float32, device=DEV) if want_smax else None
+    MW = (G + 31) // 32
+    isl = torch.full((max(P, 1) * MW,), 0x7BADBEEF, dtype=torch.int32, device=DEV) if want_slots else None
     torch.cuda.synchronize()
     r = eng.decide_ptr(u_t, P, G, T, db, power=w_t, eligible=e_t, created_ts=c_t, cutoff_ts=kw.get("cutoff_ts", 0),
                        power_threshold=thr, candidate_bits=cb, series_max=sm, veto_bits=vb, row_stride=stride,
-                       util_format=util_format)
+                       util_format=util_format, idle_slots=isl)
     W = (P + 31) // 32
     return (_u32(db)[:W], _u32(cb)[:W], (r.n_series, r.n_candidates, r.n_decisions),
-            sm.cpu().numpy()[:P * G].reshape(P, G) if want_smax else None, _u32(vb)[:W] if want_veto else None)
+            sm.cpu().numpy()[:P * G].reshape(P, G) if want_smax else None, _u32(vb)[:W] if want_veto else None,
+            _u32(isl)[:P * MW].reshape(P, MW) if want_slots else None)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -154,33 +169,45 @@ def test_knob_sets_cover_every_value():
     assert {p for _, _, p in KNOB_SETS} == {0, 1} and {v for _, v, _ in KNOB_SETS} == {"tma", "ldg", "auto"}
 
 
+def _modes(kernel):
+    """read modes a knob set decides in: whole (series_max) always; early (idle_slots, no series_max) for AUTO, whose
+    kernel it changes"""
+    return (False, True) if kernel == "auto" else (False,)
+
+
 @pytest.mark.parametrize("ks", KNOB_SETS, ids=SET_IDS)
 def test_knob_set_random_and_strided_windows(ks, sm_count, plan_exe, oracle_c):
     knobs, kernel, pdl = ks
     knobs = dataclasses.replace(knobs, sm_count=sm_count)
     eng = _engine(knobs, kernel, pdl)
     try:
-        for P, G, T in SHAPES:
-            for opts in ((False, False), (True, True)):
-                rng = np.random.default_rng(P * 31 + G * 7 + T)
-                u, kw = _random_window(rng, P, G, T, *opts)
-                exp = oracle_c.decide(u, **kw)
-                _assert_intended(plan_exe, knobs, kernel, T, P * G * (2 if opts[0] else 1), P, tma_ok=T % 4 == 0)
-                u_t = torch.from_numpy(u).to(DEV)
-                w_t = torch.from_numpy(kw["power"]).to(DEV) if opts[0] else None
-                bits, cbits, counts, smax, _ = _device_decide(eng, u_t, P, G, T, w_t, kw, kw.get("power_threshold", 0.0))
-                _check(bits, cbits, counts, exp, smax)
-        for T, stride, offset in [(100, 104, 0), (100, 101, 0), (97, 97, 1), (64, 64, 3), (1800, 1800, 2),
-                                  (1800, 1816, 0), (33, 40, 1)]:
-            P, G = 130, 4
-            rng = np.random.default_rng(T * 7 + stride + offset)
-            u, _ = _random_window(rng, P, G, T, False, False)
-            buf = np.full(offset + P * G * stride + 8, 99.0, np.float32)    # poisoned padding and slack
-            buf[offset: offset + P * G * stride].reshape(P * G, stride)[:, :T] = u.reshape(P * G, T)
-            t = torch.from_numpy(buf).to(DEV)
-            _assert_intended(plan_exe, knobs, kernel, T, P * G, P, tma_ok=T % 4 == 0 and stride % 4 == 0 and offset == 0)
-            bits, cbits, counts, smax, _ = _device_decide(eng, t[offset:].data_ptr(), P, G, T, stride=stride)
-            _check(bits, cbits, counts, oracle_c.decide(u), smax)
+        for early in _modes(kernel):
+            for P, G, T in SHAPES:
+                for opts in ((False, False), (True, True)):
+                    rng = np.random.default_rng(P * 31 + G * 7 + T)
+                    u, kw = _random_window(rng, P, G, T, *opts)
+                    exp = oracle_c.decide(u, **kw)
+                    _assert_intended(plan_exe, knobs, kernel, T, P * G * (2 if opts[0] else 1), P, tma_ok=T % 4 == 0,
+                                     may_stop=early)
+                    u_t = torch.from_numpy(u).to(DEV)
+                    w_t = torch.from_numpy(kw["power"]).to(DEV) if opts[0] else None
+                    bits, cbits, counts, smax, _, isl = _device_decide(eng, u_t, P, G, T, w_t, kw,
+                                                                       kw.get("power_threshold", 0.0),
+                                                                       want_smax=not early, want_slots=early)
+                    _check(bits, cbits, counts, exp, smax, islots=isl)
+            for T, stride, offset in [(100, 104, 0), (100, 101, 0), (97, 97, 1), (64, 64, 3), (1800, 1800, 2),
+                                      (1800, 1816, 0), (33, 40, 1)]:
+                P, G = 130, 4
+                rng = np.random.default_rng(T * 7 + stride + offset)
+                u, _ = _random_window(rng, P, G, T, False, False)
+                buf = np.full(offset + P * G * stride + 8, 99.0, np.float32)    # poisoned padding and slack
+                buf[offset: offset + P * G * stride].reshape(P * G, stride)[:, :T] = u.reshape(P * G, T)
+                t = torch.from_numpy(buf).to(DEV)
+                _assert_intended(plan_exe, knobs, kernel, T, P * G, P,
+                                 tma_ok=T % 4 == 0 and stride % 4 == 0 and offset == 0, may_stop=early)
+                bits, cbits, counts, smax, _, isl = _device_decide(eng, t[offset:].data_ptr(), P, G, T, stride=stride,
+                                                                   want_smax=not early, want_slots=early)
+                _check(bits, cbits, counts, oracle_c.decide(u), smax, islots=isl)
     finally:
         eng.close()
 
@@ -197,14 +224,16 @@ def test_knob_set_host_window_in_many_chunks(ks, sm_count, plan_exe, oracle_c):
         u, kw = _random_window(rng, P, G, T, True, True)
         chunk_pods = (1 << 20) // (G * T * 8)
         assert (P + chunk_pods - 1) // chunk_pods >= 15
-        _assert_intended(plan_exe, knobs, kernel, T, chunk_pods * G * 2, P)
-        d = eng.decide(u, kw["power"], kw["eligible"], kw["created_ts"], kw["cutoff_ts"], kw["power_threshold"],
-                       want_series_max=True, want_veto=True)
         exp = oracle_c.decide(u, **kw)
-        _check(d.decision_bits, d.candidate_bits, (d.n_series, d.n_candidates, d.n_decisions), exp, d.series_max)
         from oracle import oracle_np
-        assert np.array_equal(d.veto_bits, oracle_np.decide(u, kw["power"], kw["eligible"], kw["created_ts"],
-                                                            kw["cutoff_ts"], kw["power_threshold"])["veto_bits"])
+        exp["veto_bits"] = oracle_np.decide(u, kw["power"], kw["eligible"], kw["created_ts"], kw["cutoff_ts"],
+                                            kw["power_threshold"])["veto_bits"]
+        for early in _modes(kernel):
+            _assert_intended(plan_exe, knobs, kernel, T, chunk_pods * G * 2, P, may_stop=early)
+            d = eng.decide(u, kw["power"], kw["eligible"], kw["created_ts"], kw["cutoff_ts"], kw["power_threshold"],
+                           want_series_max=not early, want_veto=True, want_idle_slots=early)
+            _check(d.decision_bits, d.candidate_bits, (d.n_series, d.n_candidates, d.n_decisions), exp, d.series_max,
+                   d.veto_bits, d.idle_slots)
     finally:
         eng.close()
 
@@ -246,7 +275,7 @@ def test_knob_set_batch_of_unlike_decisions(ks, sm_count, plan_exe, oracle_c):
             if smax:
                 c["series_max"] = torch.full((P * G,), -777.0, dtype=torch.float32, device=DEV)
             rows = P * G * (2 if power else 1)
-            _assert_intended(plan_exe, knobs, kernel, T, rows, P, tma_ok=T % 4 == 0, util_u8=u8)
+            _assert_intended(plan_exe, knobs, kernel, T, rows, P, tma_ok=T % 4 == 0, util_u8=u8, may_stop=not smax)
             calls.append(c)
             keep.append((u, kw))
         batch = eng.make_batch(calls)
@@ -292,20 +321,22 @@ def _synth(eng, seed, P, G, T, power):
 
 @pytest.mark.parametrize("P,fold_threads", [(140_000, 256), (250_000, 256), (40_000, 64)])
 def test_scale_fold_loops(P, fold_threads, sm_count, plan_exe, oracle_c):
-    """fold rounds > 1 at the default tilings (and 64-thread fold CTAs), both kernels, power and eligibility; every
-    row checked through series_max and the veto bits"""
+    """fold rounds > 1 at the default tilings (and 64-thread fold CTAs), power and eligibility: tma and ldg reading
+    every row whole, every row checked through series_max; the probe kernel (auto, rows stop early) with every row
+    checked through idle_slots, which the fold (k_fold<false, true>) writes; the veto bits always"""
     G, T, seed = 4, 1800, 0x5EED0004 + P
     _need(2 * P * G * T * 4, f"{P} x {G} x {T} with power")
     knobs = K(sm_count=sm_count, fold_threads=fold_threads)
     exp = _oracle_synth(oracle_c, seed, P, G, T, True)
-    for kernel in ("tma", "ldg"):
+    for kernel, early in (("tma", False), ("ldg", False), ("auto", True)):
         eng = _engine(knobs, kernel)
         try:
-            p = _assert_intended(plan_exe, knobs, kernel, T, 2 * P * G, P)
+            p = _assert_intended(plan_exe, knobs, kernel, T, 2 * P * G, P, may_stop=early)
             assert p.fold_rounds >= 2, p
             u, w, e = _synth(eng, seed, P, G, T, True)
-            out = _device_decide(eng, u, P, G, T, w, {"eligible": e.cpu().numpy()}, 150.0, want_veto=True)
-            _check(*out[:3], exp, out[3], out[4])
+            out = _device_decide(eng, u, P, G, T, w, {"eligible": e.cpu().numpy()}, 150.0, want_veto=True,
+                                 want_smax=not early, want_slots=early)
+            _check(*out[:3], exp, out[3], out[4], out[5])
             assert 0 < out[2][2] < P
             del u, w, e
         finally:
@@ -328,13 +359,14 @@ def _u8_plane(eng, seed, P, G, T, pods_per_fill=20_000):
 @pytest.mark.slow
 @pytest.mark.parametrize("fmt", ["f32", "u8"])
 def test_scale_config_5_shard(fmt, sm_count, plan_exe, oracle_c):
-    """BASELINE config 5 per GPU: 312,500 x 4 x 7,200 = 9.0e9 cells, more than 2^32; the fold takes 3 rounds"""
+    """BASELINE config 5 per GPU: 312,500 x 4 x 7,200 = 9.0e9 cells, more than 2^32; the fold takes 3 rounds.  As f32
+    also with rows that stop early (AUTO: the probe kernel), every row checked through idle_slots"""
     P, G, T, seed = 312_500, 4, 7200, 0x5EED0005
     cells = P * G * T
     _need(cells * (4 if fmt == "f32" else 1) + 3 * GB, f"config 5 shard as {fmt}")
     knobs = K(sm_count=sm_count)
     exp = _oracle_synth(oracle_c, seed, P, G, T, False)
-    kernels = ("tma", "ldg") if fmt == "f32" else ("auto",)
+    legs = (("tma", False), ("ldg", False), ("auto", True)) if fmt == "f32" else (("auto", False),)
     eng = _engine(knobs, "auto")
     try:
         if fmt == "f32":
@@ -345,14 +377,14 @@ def test_scale_config_5_shard(fmt, sm_count, plan_exe, oracle_c):
         e = torch.empty(P, dtype=torch.uint8, device=DEV)
         eng.synth_eligible(seed, e, 0, P)
         torch.cuda.synchronize()
-        for kernel in kernels:
+        for kernel, early in legs:
             k_eng = eng if kernel == "auto" else _engine(knobs, kernel)
             try:
-                p = _assert_intended(plan_exe, knobs, kernel, T, P * G, P, util_u8=fmt == "u8")
+                p = _assert_intended(plan_exe, knobs, kernel, T, P * G, P, util_u8=fmt == "u8", may_stop=early)
                 assert p.fold_rounds >= 3, p
                 out = _device_decide(k_eng, u, P, G, T, None, {"eligible": e.cpu().numpy()},
-                                     util_format=1 if fmt == "u8" else 0)
-                _check(*out[:3], exp, out[3])
+                                     util_format=1 if fmt == "u8" else 0, want_smax=not early, want_slots=early)
+                _check(*out[:3], exp, out[3], None, out[5])
             finally:
                 if k_eng is not eng:
                     k_eng.close()
@@ -364,23 +396,37 @@ def test_scale_config_5_shard(fmt, sm_count, plan_exe, oracle_c):
 # ---------------------------------------------------------------------------------------------
 # the series limit: 2^31 - 32 series with a power plane = 2^32 - 64 rows in one reduce launch
 # ---------------------------------------------------------------------------------------------
+def _check_idle_slots_synth(oracle_c, islots, seed, P, G, T, pods_per_slice=1 << 21):
+    """idle_slots of a synthetic window against the oracle's row maxima, one slice of pods at a time (the maxima of
+    every series at the series limit would take 8 GB of host memory)"""
+    for p0 in range(0, P, pods_per_slice):
+        n = min(pods_per_slice, P - p0)
+        smax = oracle_c.decide_synth(seed, p0, n, G, T, want_series_max=True)["series_max"]
+        check_idle_slots(islots[p0:p0 + n], smax)
+
+
 @pytest.mark.slow
-@pytest.mark.parametrize("kernel,T", [("ldg", 1), ("tma", 4)])
+@pytest.mark.parametrize("kernel,T", [("ldg", 1), ("tma", 4), ("auto", 4)])
 def test_series_limit_with_power(kernel, T, sm_count, plan_exe, oracle_c):
+    """ldg and tma ask for no series_max and stop rows early; auto does the same with the probe kernel, on sm_count
+    CTAs, every row checked through idle_slots"""
     P, G, seed = 67_108_863, 32, 0x5EED0006
     S = P * G
     assert S == 2**31 - 32
-    _need(2 * S * T * 4, f"the series limit at T = {T}")
+    early_slots = kernel == "auto"
+    _need(2 * S * T * 4 + (P * 4 if early_slots else 0), f"the series limit at T = {T}")
     knobs = K(sm_count=sm_count)
-    p = _assert_intended(plan_exe, knobs, kernel, T, 2 * S, P)
+    p = _assert_intended(plan_exe, knobs, kernel, T, 2 * S, P, may_stop=True)
     assert p.grid == (2 * sm_count if kernel == "ldg" else sm_count), p
     exp = _oracle_synth(oracle_c, seed, P, G, T, True, smax=False)
     eng = _engine(knobs, kernel)
     try:
         u, w, e = _synth(eng, seed, P, G, T, True)
         out = _device_decide(eng, u, P, G, T, w, {"eligible": e.cpu().numpy()}, 150.0, want_smax=False,
-                             want_veto=True)
+                             want_veto=True, want_slots=early_slots)
         _check(*out[:3], exp, None, out[4])
+        if early_slots:
+            _check_idle_slots_synth(oracle_c, out[5], seed, P, G, T)
         del u, w, e
     finally:
         eng.close()

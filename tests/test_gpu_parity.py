@@ -3,6 +3,13 @@
 Bit-exact on the decision / candidate bitmaps and the three counts; series_max numerically
 exact (tolerance 0; -0.0 == +0.0, NaN matches NaN — the fmax tree does not preserve which
 signed zero came first, Prometheus' sequential fold does; the verdict is unaffected).
+
+Most windows are decided in two read modes.  "whole" asks for series_max, so every kernel reads
+every row to its end.  "early" asks for idle_slots and no series_max, the call the gpu-pruner
+binary makes: rows stop at their first settling sample, and AUTO runs the probe kernel
+(k_reduce_probe) when the rows can be bulk-copied, else the early-exit LDG kernel.  idle_slots
+is the per-row output that keeps early exit on, so every row's verdict is checked word for word,
+not only the per-pod bitmaps where another row of the same pod could hide a wrong one.
 """
 import ctypes as C
 import os
@@ -10,13 +17,18 @@ import os
 import numpy as np
 import pytest
 
+import geometry
 import kat
 
 pytestmark = pytest.mark.gpu
 
 torch = pytest.importorskip("torch")
 KATS = kat.all_kats()
-VARIANTS = ["ldg", "tma"]
+VARIANTS = ["ldg", "tma", "auto"]
+MODES = ["whole", "early"]
+# (kernel variant, read mode); a whole-row call is named by its variant alone
+VARIANT_MODES = [(v, m) for v in VARIANTS for m in MODES]
+VM_IDS = [v if m == "whole" else f"{v}-{m}" for v, m in VARIANT_MODES]
 
 
 @pytest.fixture(scope="module")
@@ -31,17 +43,67 @@ def engines():
         x.close()
 
 
-def _check(res_bits, res_cbits, counts, exp, smax=None):
+@pytest.fixture(scope="module")
+def plan_exe(tmp_path_factory):
+    return geometry.build(tmp_path_factory.mktemp("launch_plan"))
+
+
+def expected_idle_slots(series_max):
+    """gpr_result.idle_slots without a group table (include/gpr.h): bit g of pod p's ceil(G / 32) words is set iff
+    row g's window max is == 0 (-0.0 counts, NaN — no sample — does not); the bits above G are 0"""
+    smax = np.asarray(series_max, np.float32)
+    P, G = smax.shape
+    MW = (G + 31) // 32
+    idle = np.zeros((P, MW * 32), bool)
+    idle[:, :G] = smax == 0
+    return np.packbits(idle.reshape(P, MW, 32), axis=-1, bitorder="little").view("<u4").reshape(P, MW)
+
+
+def check_idle_slots(islots, series_max):
+    want = expected_idle_slots(series_max)
+    got = np.asarray(islots).view(np.uint32).reshape(want.shape)
+    bad = np.argwhere(got != want)
+    assert bad.size == 0, (f"idle_slots differ from the oracle at pod {bad[0][0]} word {bad[0][1]}: "
+                           f"{int(got[tuple(bad[0])]):#010x} != {int(want[tuple(bad[0])]):#010x}")
+
+
+def _check(res_bits, res_cbits, counts, exp, smax=None, islots=None):
     assert np.array_equal(res_bits, exp["decision_bits"]), "decision bitmap differs from oracle"
     assert np.array_equal(res_cbits, exp["candidate_bits"]), "candidate bitmap differs from oracle"
     assert counts == (exp["n_series"], exp["n_candidates"], exp["n_decisions"])
     if smax is not None:
         assert kat.smax_equal(smax, exp["series_max"])
+    if islots is not None:
+        check_idle_slots(islots, exp["series_max"])
+
+
+def _outputs(mode):
+    """the outputs a call asks for in the given read mode"""
+    assert mode in MODES
+    return {"want_smax": mode == "whole", "want_slots": mode == "early"}
+
+
+def assert_ran(plan_exe, sm_count, variant, mode, T, rows, tma_ok=True, P=1):
+    """the geometry header's verdict for this call (gpu-pruner_b200/csrc/gpr_launch.h, which gpr_api.cu launches):
+    rows that cannot be bulk-copied take LDG; an early AUTO call the probe kernel, a whole one k_reduce_tma"""
+    p = geometry.plan(plan_exe, geometry.Knobs(sm_count=sm_count), variant, T, rows, tma_ok, False, P,
+                      mode == "early")
+    if variant == "ldg" or not tma_ok:
+        want = "ldg"
+    else:
+        want = "probe" if variant == "auto" and mode == "early" else "tma"
+    assert p.kernel == want, (variant, mode, p)
+    return p
+
+
+@pytest.fixture(scope="module")
+def sm_count(engines):
+    return engines["ldg"].device_info()["sm_count"]
 
 
 def _device_decide(eng, u, power=None, eligible=None, created=None, cutoff=0, thr=0.0, stride=0,
-                   want_smax=True, u_t=None, w_t=None):
-    """window already on the device (torch tensors) -> numpy results"""
+                   want_smax=True, u_t=None, w_t=None, want_slots=False):
+    """window already on the device (torch tensors) -> numpy results (idle_slots last, [P, ceil(G / 32)])"""
     dev = "cuda:0"
     P, G, T = u.shape if u_t is None else (u_t.shape[0], u_t.shape[1], u_t.shape[2])
     if u_t is None:
@@ -54,41 +116,64 @@ def _device_decide(eng, u, power=None, eligible=None, created=None, cutoff=0, th
     db = torch.full((W,), 0x7BADBEEF, dtype=torch.int32, device=dev)
     cb = torch.full((W,), 0x7BADBEEF, dtype=torch.int32, device=dev)
     sm = torch.full((max(P * G, 1),), -777.0, dtype=torch.float32, device=dev) if want_smax else None
+    MW = (G + 31) // 32
+    isl = torch.full((max(P, 1) * MW,), 0x7BADBEEF, dtype=torch.int32, device=dev) if want_slots else None
     torch.cuda.synchronize()
     r = eng.decide_ptr(u_t, P, G, T, db, power=w_t, eligible=e_t, created_ts=c_t, cutoff_ts=cutoff,
-                       power_threshold=thr, candidate_bits=cb, series_max=sm, row_stride=stride)
+                       power_threshold=thr, candidate_bits=cb, series_max=sm, row_stride=stride, idle_slots=isl)
     W = (P + 31) // 32
     bits = db.cpu().numpy().view(np.uint32)[:W]
     cbits = cb.cpu().numpy().view(np.uint32)[:W]
     smax = sm.cpu().numpy()[: P * G].reshape(P, G) if want_smax else None
-    return bits, cbits, (r.n_series, r.n_candidates, r.n_decisions), smax, r
+    islots = isl.cpu().numpy().view(np.uint32)[: P * MW].reshape(P, MW) if want_slots else None
+    return bits, cbits, (r.n_series, r.n_candidates, r.n_decisions), smax, r, islots
 
 
 # ---------------------------------------------------------------------------------------------
 # known-answer vectors, both kernels, host and device windows
 # ---------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("variant", VARIANTS)
+def _kat_smax(k, oracle_c):
+    """the row maxima the KAT writes out, else the oracle's"""
+    if k.series_max is not None:
+        return k.series_max
+    return oracle_c.decide(k.util, k.power, k.eligible, k.created_ts, k.cutoff_ts, k.power_threshold)["series_max"]
+
+
+def _kat_rows(k):
+    P, G, _ = k.util.shape
+    return P * G * (2 if k.power is not None and k.power_threshold else 1)
+
+
+@pytest.mark.parametrize("variant,mode", VARIANT_MODES, ids=VM_IDS)
 @pytest.mark.parametrize("k", KATS, ids=[k.name for k in KATS])
-def test_kat_host_window(k, variant, engines):
+def test_kat_host_window(k, variant, mode, engines, oracle_c, plan_exe, sm_count):
+    assert_ran(plan_exe, sm_count, variant, mode, k.util.shape[2], _kat_rows(k), k.util.shape[2] % 4 == 0)
     d = engines[variant].decide(k.util, k.power, k.eligible, k.created_ts, k.cutoff_ts,
-                                k.power_threshold, want_series_max=True)
+                                k.power_threshold, want_series_max=mode == "whole",
+                                want_idle_slots=mode == "early")
     assert np.array_equal(d.candidate_bits, kat.expected_bits(k.candidate)), k.why
     assert np.array_equal(d.decision_bits, kat.expected_bits(k.decision)), k.why
     assert (d.n_candidates, d.n_decisions) == (sum(k.candidate), sum(k.decision))
-    if k.series_max is not None:
+    if mode == "early":
+        check_idle_slots(d.idle_slots, _kat_smax(k, oracle_c))
+    elif k.series_max is not None:
         assert kat.smax_equal(d.series_max, k.series_max)
     if k.n_series is not None:
         assert d.n_series == k.n_series
 
 
-@pytest.mark.parametrize("variant", VARIANTS)
+@pytest.mark.parametrize("variant,mode", VARIANT_MODES, ids=VM_IDS)
 @pytest.mark.parametrize("k", KATS, ids=[k.name for k in KATS])
-def test_kat_device_window(k, variant, engines):
-    bits, cbits, counts, smax, _ = _device_decide(engines[variant], k.util, k.power, k.eligible,
-                                                  k.created_ts, k.cutoff_ts, k.power_threshold)
+def test_kat_device_window(k, variant, mode, engines, oracle_c, plan_exe, sm_count):
+    assert_ran(plan_exe, sm_count, variant, mode, k.util.shape[2], _kat_rows(k), k.util.shape[2] % 4 == 0)
+    bits, cbits, counts, smax, _, islots = _device_decide(engines[variant], k.util, k.power, k.eligible,
+                                                          k.created_ts, k.cutoff_ts, k.power_threshold,
+                                                          **_outputs(mode))
     assert np.array_equal(cbits, kat.expected_bits(k.candidate)), k.why
     assert np.array_equal(bits, kat.expected_bits(k.decision)), k.why
-    if k.series_max is not None:
+    if mode == "early":
+        check_idle_slots(islots, _kat_smax(k, oracle_c))
+    elif k.series_max is not None:
         assert kat.smax_equal(smax, k.series_max)
 
 
@@ -120,38 +205,41 @@ SHAPES = [(1, 1, 1), (3, 2, 5), (31, 4, 33), (64, 1, 450), (257, 8, 100), (1000,
           (999, 3, 1801), (4097, 4, 64), (50, 4, 7200), (20, 2, 9000), (6, 1, 20000)]
 
 
-@pytest.mark.parametrize("variant", VARIANTS)
+@pytest.mark.parametrize("variant,mode", VARIANT_MODES, ids=VM_IDS)
 @pytest.mark.parametrize("P,G,T", SHAPES)
 @pytest.mark.parametrize("opts", [(False, False), (True, True)])
-def test_random_device_window(P, G, T, opts, variant, engines, oracle_c, oracle_np):
+def test_random_device_window(P, G, T, opts, variant, mode, engines, oracle_c, oracle_np, plan_exe, sm_count):
     rng = np.random.default_rng(P * 31 + G * 7 + T)
     u, kw = _random_window(rng, P, G, T, *opts)
     exp = oracle_c.decide(u, **kw)
     exp2 = oracle_np.decide(u, **kw)
     assert np.array_equal(exp["decision_bits"], exp2["decision_bits"])
-    bits, cbits, counts, smax, _ = _device_decide(
+    assert_ran(plan_exe, sm_count, variant, mode, T, P * G * (2 if opts[0] else 1), T % 4 == 0)
+    bits, cbits, counts, smax, _, islots = _device_decide(
         engines[variant], u, kw.get("power"), kw.get("eligible"), kw.get("created_ts"),
-        kw.get("cutoff_ts", 0), kw.get("power_threshold", 0.0))
-    _check(bits, cbits, counts, exp, smax)
+        kw.get("cutoff_ts", 0), kw.get("power_threshold", 0.0), **_outputs(mode))
+    _check(bits, cbits, counts, exp, smax, islots)
 
 
-@pytest.mark.parametrize("variant", VARIANTS)
+@pytest.mark.parametrize("variant,mode", VARIANT_MODES, ids=VM_IDS)
 @pytest.mark.parametrize("P,G,T", [(3, 2, 5), (257, 8, 100), (1000, 4, 180), (999, 3, 1801), (300, 4, 2048)])
-def test_random_host_window(P, G, T, variant, engines, oracle_c):
+def test_random_host_window(P, G, T, variant, mode, engines, oracle_c, plan_exe, sm_count):
     rng = np.random.default_rng(P + T)
     u, kw = _random_window(rng, P, G, T, True, True)
     exp = oracle_c.decide(u, **kw)
+    assert_ran(plan_exe, sm_count, variant, mode, T, 2 * P * G, T % 4 == 0)
     d = engines[variant].decide(u, kw["power"], kw["eligible"], kw["created_ts"], kw["cutoff_ts"],
-                                kw["power_threshold"], want_series_max=True)
+                                kw["power_threshold"], want_series_max=mode == "whole",
+                                want_idle_slots=mode == "early")
     _check(d.decision_bits, d.candidate_bits, (d.n_series, d.n_candidates, d.n_decisions), exp,
-           d.series_max)
+           d.series_max, d.idle_slots)
     assert d.kernel_ms > 0
 
 
-@pytest.mark.parametrize("variant", VARIANTS)
+@pytest.mark.parametrize("variant,mode", VARIANT_MODES, ids=VM_IDS)
 @pytest.mark.parametrize("T,stride,offset", [(100, 104, 0), (100, 101, 0), (97, 97, 1), (64, 64, 3),
                                              (1800, 1800, 2), (1800, 1816, 0), (33, 40, 1)])
-def test_strided_and_misaligned_rows(T, stride, offset, variant, engines, oracle_c):
+def test_strided_and_misaligned_rows(T, stride, offset, variant, mode, engines, oracle_c, plan_exe, sm_count):
     """row_stride > T and bases that are only 4-byte aligned: the head/tail peel must read every
     sample exactly once and never a neighbour's"""
     P, G = 130, 4
@@ -164,15 +252,18 @@ def test_strided_and_misaligned_rows(T, stride, offset, variant, engines, oracle
     t = torch.from_numpy(buf).to("cuda:0")
     u_t = t[offset:]
     exp = oracle_c.decide(u)
+    assert_ran(plan_exe, sm_count, variant, mode, T, P * G, T % 4 == 0 and stride % 4 == 0 and offset == 0)
     W = (P + 31) // 32
     db = torch.zeros(W, dtype=torch.int32, device="cuda:0")
     cb = torch.zeros(W, dtype=torch.int32, device="cuda:0")
-    sm = torch.zeros(P * G, dtype=torch.float32, device="cuda:0")
+    sm = torch.zeros(P * G, dtype=torch.float32, device="cuda:0") if mode == "whole" else None
+    isl = torch.full((P,), 0x7BADBEEF, dtype=torch.int32, device="cuda:0") if mode == "early" else None
     torch.cuda.synchronize()   # the engine's stream is not ordered with torch's: buffers must be ready
     r = engines[variant].decide_ptr(u_t.data_ptr(), P, G, T, db, candidate_bits=cb, series_max=sm,
-                                    row_stride=stride)
+                                    row_stride=stride, idle_slots=isl)
     _check(db.cpu().numpy().view(np.uint32), cb.cpu().numpy().view(np.uint32),
-           (r.n_series, r.n_candidates, r.n_decisions), exp, sm.cpu().numpy().reshape(P, G))
+           (r.n_series, r.n_candidates, r.n_decisions), exp,
+           None if sm is None else sm.cpu().numpy().reshape(P, G), None if isl is None else isl.cpu().numpy())
 
 
 # ---------------------------------------------------------------------------------------------
@@ -204,22 +295,27 @@ def _synth_device(eng, seed, P, G, T, power, off=0):
     return u, w, e
 
 
-@pytest.mark.parametrize("variant", VARIANTS)
+@pytest.mark.parametrize("variant,mode", VARIANT_MODES, ids=VM_IDS)
 @pytest.mark.parametrize("power", [False, True])
-def test_config_c2_full_parity(variant, power, engines, oracle_c):
-    """BASELINE config #2: 10k pods x 4 GPUs x 1800 samples, every bit against the oracle"""
+def test_config_c2_full_parity(variant, power, mode, engines, oracle_c, plan_exe, sm_count):
+    """BASELINE config #2: 10k pods x 4 GPUs x 1800 samples, every bit (and every row's max or idle slot) against
+    the oracle"""
     seed, P, G, T = 0x5EED0002, 10000, 4, 1800
     eng = engines[variant]
     u, w, e = _synth_device(eng, seed, P, G, T, power)
-    exp = oracle_c.decide_synth(seed, 0, P, G, T, use_power=power, power_threshold=150.0, use_elig=True)
-    bits, cbits, counts, _, r = _device_decide(eng, None, u_t=u, w_t=w, eligible=e.cpu().numpy(),
-                                               thr=150.0 if power else 0.0, want_smax=False)
-    _check(bits, cbits, counts, exp)
+    exp = oracle_c.decide_synth(seed, 0, P, G, T, use_power=power, power_threshold=150.0, use_elig=True,
+                                want_series_max=True)
+    assert_ran(plan_exe, sm_count, variant, mode, T, P * G * (2 if power else 1))
+    bits, cbits, counts, smax, r, islots = _device_decide(eng, None, u_t=u, w_t=w, eligible=e.cpu().numpy(),
+                                                          thr=150.0 if power else 0.0, **_outputs(mode))
+    _check(bits, cbits, counts, exp, smax, islots)
     assert 0 < counts[2] < P
     # and through the host-window path (pinned staging, chunked H2D overlapped with the reduce)
     d = eng.decide(u.cpu().numpy(), None if w is None else w.cpu().numpy(), e.cpu().numpy(),
-                   power_threshold=150.0 if power else 0.0)
-    _check(d.decision_bits, d.candidate_bits, (d.n_series, d.n_candidates, d.n_decisions), exp)
+                   power_threshold=150.0 if power else 0.0, want_series_max=mode == "whole",
+                   want_idle_slots=mode == "early")
+    _check(d.decision_bits, d.candidate_bits, (d.n_series, d.n_candidates, d.n_decisions), exp, d.series_max,
+           d.idle_slots)
 
 
 def test_config_c1_golden_fixture(engines):
@@ -228,48 +324,50 @@ def test_config_c1_golden_fixture(engines):
     seed, P, G, T = int(gold["seed"]), int(gold["P"]), int(gold["G"]), int(gold["T"])
     for v in VARIANTS:
         u, w, e = _synth_device(engines[v], seed, P, G, T, True)
-        bits, cbits, counts, _, _ = _device_decide(engines[v], None, u_t=u, eligible=e.cpu().numpy(),
-                                                   want_smax=False)
+        bits, cbits, counts, _, _, _ = _device_decide(engines[v], None, u_t=u, eligible=e.cpu().numpy(),
+                                                      want_smax=False)
         assert np.array_equal(bits, gold["decision_bits"]) and np.array_equal(cbits, gold["candidate_bits"])
-        bits, cbits, counts, _, _ = _device_decide(engines[v], None, u_t=u, w_t=w, thr=150.0,
-                                                   eligible=e.cpu().numpy(), want_smax=False)
+        bits, cbits, counts, _, _, _ = _device_decide(engines[v], None, u_t=u, w_t=w, thr=150.0,
+                                                      eligible=e.cpu().numpy(), want_smax=False)
         assert np.array_equal(bits, gold["decision_bits_power"])
         assert list(np.flatnonzero(np.unpackbits(bits.view(np.uint8), bitorder="little"))) == \
             list(gold["idle_pods_power"])
 
 
 @pytest.mark.slow
-@pytest.mark.parametrize("variant", VARIANTS)
-def test_config_c3_full_parity_and_properties(variant, engines, oracle_c):
+@pytest.mark.parametrize("variant,mode", VARIANT_MODES, ids=VM_IDS)
+def test_config_c3_full_parity_and_properties(variant, mode, engines, oracle_c, plan_exe, sm_count):
     """BASELINE config #3: 100k x 8 x 3600 (11.5 GB).  Full parity by streaming regeneration on the
-    host, plus size-independent properties: idempotence, shard consistency, time-reversal
-    invariance (max is order independent), monotonicity, counts == popcounts."""
+    host, every row through series_max or idle_slots, plus size-independent properties: idempotence,
+    shard consistency, time-reversal invariance (max is order independent), monotonicity, counts ==
+    popcounts."""
     seed, P, G, T = 0x5EED0003, 100000, 8, 3600
     eng = engines[variant]
     u, _, e = _synth_device(eng, seed, P, G, T, False)
     en = e.cpu().numpy()
-    bits, cbits, counts, _, _ = _device_decide(eng, None, u_t=u, eligible=en, want_smax=False)
-    exp = oracle_c.decide_synth(seed, 0, P, G, T, use_elig=True)
-    _check(bits, cbits, counts, exp)
+    assert_ran(plan_exe, sm_count, variant, mode, T, P * G)
+    bits, cbits, counts, smax, _, islots = _device_decide(eng, None, u_t=u, eligible=en, **_outputs(mode))
+    exp = oracle_c.decide_synth(seed, 0, P, G, T, use_elig=True, want_series_max=True)
+    _check(bits, cbits, counts, exp, smax, islots)
     pop = lambda b: int(np.unpackbits(b.view(np.uint8)).sum())
     assert counts[1] == pop(cbits) and counts[2] == pop(bits)
     assert np.all(bits & ~cbits == 0)                       # decision implies candidate
     # idempotence
-    bits2, cbits2, counts2, _, _ = _device_decide(eng, None, u_t=u, eligible=en, want_smax=False)
+    bits2, cbits2, counts2, _, _, _ = _device_decide(eng, None, u_t=u, eligible=en, want_smax=False)
     assert np.array_equal(bits, bits2) and counts == counts2
     # shard consistency: a 32-aligned slice of the window gives the same words
     p0, p1 = 32 * 1000, 32 * 2200
-    sb, scb, _, _, _ = _device_decide(eng, None, u_t=u[p0:p1], eligible=en[p0:p1], want_smax=False)
+    sb, scb, _, _, _, _ = _device_decide(eng, None, u_t=u[p0:p1], eligible=en[p0:p1], want_smax=False)
     assert np.array_equal(sb, bits[p0 // 32: p1 // 32]) and np.array_equal(scb, cbits[p0 // 32: p1 // 32])
     # time reversal
     sub = u[:20000].flip(2).contiguous()
-    rb, rcb, _, _, _ = _device_decide(eng, None, u_t=sub, eligible=en[:20000], want_smax=False)
+    rb, rcb, _, _, _, _ = _device_decide(eng, None, u_t=sub, eligible=en[:20000], want_smax=False)
     assert np.array_equal(rb, bits[:625]) and np.array_equal(rcb, cbits[:625])
     # monotonicity: poke one positive sample into 1000 random series -> bits can only clear
     g = torch.Generator(device="cpu").manual_seed(1)
     pods = torch.randint(0, P, (1000,), generator=g)
     u[pods, torch.randint(0, G, (1000,), generator=g), torch.randint(0, T, (1000,), generator=g)] = 9.0
-    mb, mcb, _, _, _ = _device_decide(eng, None, u_t=u, eligible=en, want_smax=False)
+    mb, mcb, _, _, _, _ = _device_decide(eng, None, u_t=u, eligible=en, want_smax=False)
     assert np.all(mcb & ~cbits == 0) and not np.array_equal(mcb, cbits)
 
 
@@ -318,9 +416,15 @@ def test_batch_entry_point(variant, engines, oracle_c):
                (r.n_series, r.n_candidates, r.n_decisions), exp)
 
 
+def resident_ld(T, block_index):
+    """the row length gpr_decide_resident decides on: the ring's T, or the block index's idx_ld = ceil(T / 64)
+    rounded up to a multiple of 4"""
+    return (-(-T // 64) + 3) // 4 * 4 if block_index else T
+
+
 @pytest.mark.parametrize("block_index", [False, True], ids=["rescan", "block-index"])
-@pytest.mark.parametrize("variant", VARIANTS)
-def test_resident_window_ring(variant, block_index, engines, oracle_c):
+@pytest.mark.parametrize("variant,mode", VARIANT_MODES, ids=VM_IDS)
+def test_resident_window_ring(variant, block_index, mode, engines, oracle_c, plan_exe, sm_count):
     """daemon mode: append columns tick by tick into the HBM ring, rescan, compare with the
     oracle on the window a fresh range query would have returned"""
     eng = engines[variant]
@@ -329,23 +433,25 @@ def test_resident_window_ring(variant, block_index, engines, oracle_c):
     full = oracle_c.synth_fill(seed, 0, 0, P, G, total)       # one long history
     fullw = oracle_c.synth_fill(seed, 1, 0, P, G, total)
     eng.resident_init(P, G, T, power_plane=True, block_index=block_index)
+    assert_ran(plan_exe, sm_count, variant, mode, resident_ld(T, block_index), 2 * P * G)
     W = (P + 31) // 32
     db = np.zeros(W, np.uint32)
     cb = np.zeros(W, np.uint32)
-    sm = np.zeros((P, G), np.float32)
+    sm = np.zeros((P, G), np.float32) if mode == "whole" else None
+    isl = np.full(P, 0xDEADBEEF, np.uint32) if mode == "early" else None
     t = 0
     for n_new in (60, 1, 179, 240, 37, 300, 83):              # 300 > T: only the newest T survive
         eng.append(full[:, :, t:t + n_new], fullw[:, :, t:t + n_new])
         t += n_new
         r = eng.decide_ptr(None, 0, 0, 0, db, candidate_bits=cb, series_max=sm, power_threshold=150.0,
-                           in_kind=0, out_kind=0, resident=True)
+                           in_kind=0, out_kind=0, resident=True, idle_slots=isl)
         lo = max(0, t - T)
         win = np.full((P, G, T), np.nan, np.float32)
         win[:, :, : t - lo] = full[:, :, lo:t]
         winw = np.full((P, G, T), np.nan, np.float32)
         winw[:, :, : t - lo] = fullw[:, :, lo:t]
         exp = oracle_c.decide(win, winw, power_threshold=150.0)
-        _check(db, cb, (r.n_series, r.n_candidates, r.n_decisions), exp, sm)
+        _check(db, cb, (r.n_series, r.n_candidates, r.n_decisions), exp, sm, isl)
 
 
 @pytest.mark.parametrize("T", [64, 100, 240, 7200])
@@ -425,9 +531,9 @@ def test_native_library_is_what_ran(engines):
 # ---------------------------------------------------------------------------------------------
 # seeded fuzz over shape / stride / alignment / clause combinations, G up to the 32-slot limit
 # ---------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("variant", VARIANTS)
+@pytest.mark.parametrize("variant,mode", VARIANT_MODES, ids=VM_IDS)
 @pytest.mark.parametrize("seed", range(24))
-def test_fuzz_shapes(seed, variant, engines, oracle_c):
+def test_fuzz_shapes(seed, variant, mode, engines, oracle_c, plan_exe, sm_count):
     rng = np.random.default_rng(10_000 + seed)
     P = int(rng.choice([1, 2, 31, 32, 33, 63, 100, 257, 1000, 3000]))
     G = int(rng.choice([1, 2, 3, 4, 5, 7, 8, 16, 31, 32]))
@@ -450,18 +556,22 @@ def test_fuzz_shapes(seed, variant, engines, oracle_c):
     wt = plane(kw["power"]) if with_power else None
     et = torch.from_numpy(kw["eligible"]).to("cuda:0") if with_gates else None
     ct = torch.from_numpy(kw["created_ts"]).to("cuda:0") if with_gates else None
+    assert_ran(plan_exe, sm_count, variant, mode, T, P * G * (2 if with_power else 1),
+               T % 4 == 0 and stride % 4 == 0 and off == 0)
     W = (P + 31) // 32
     db = torch.full((W,), -1, dtype=torch.int32, device="cuda:0")
     cb = torch.full((W,), -1, dtype=torch.int32, device="cuda:0")
-    sm = torch.zeros(P * G, dtype=torch.float32, device="cuda:0")
+    sm = torch.zeros(P * G, dtype=torch.float32, device="cuda:0") if mode == "whole" else None
+    isl = torch.full((P,), -1, dtype=torch.int32, device="cuda:0") if mode == "early" else None
     torch.cuda.synchronize()
     r = engines[variant].decide_ptr(ut[off:].data_ptr(), P, G, T, db,
                                     power=None if wt is None else wt[off:].data_ptr(), eligible=et,
                                     created_ts=ct, cutoff_ts=kw.get("cutoff_ts", 0),
                                     power_threshold=kw.get("power_threshold", 0.0), candidate_bits=cb,
-                                    series_max=sm, row_stride=stride)
+                                    series_max=sm, row_stride=stride, idle_slots=isl)
     _check(db.cpu().numpy().view(np.uint32), cb.cpu().numpy().view(np.uint32),
-           (r.n_series, r.n_candidates, r.n_decisions), exp, sm.cpu().numpy().reshape(P, G))
+           (r.n_series, r.n_candidates, r.n_decisions), exp,
+           None if sm is None else sm.cpu().numpy().reshape(P, G), None if isl is None else isl.cpu().numpy())
 
 
 def test_gpu_slot_limit(engines):
@@ -471,18 +581,19 @@ def test_gpu_slot_limit(engines):
     P, G, T = 40, 32, 16
     u = np.full((P, G, T), 5.0, np.float32)
     u[:, 31, :] = 0.0
-    bits, cbits, counts, smax, _ = _device_decide(eng, u)
+    bits, cbits, counts, smax, _, _ = _device_decide(eng, u)
     assert counts == (P, P, P) and int(np.unpackbits(cbits.view(np.uint8)).sum()) == P
     with pytest.raises(g.GprError) as ei:
         eng.decide(np.zeros((2, 257, 4), np.float32))
     assert ei.value.code == g.ffi.GPR_E_UNSUPPORTED
 
 
-@pytest.mark.parametrize("variant", VARIANTS)
+@pytest.mark.parametrize("variant,mode", VARIANT_MODES, ids=VM_IDS)
 @pytest.mark.parametrize("G", [33, 64, 65, 100, 256])
-def test_pods_with_more_than_32_series_slots(G, variant, engines, oracle_c):
+def test_pods_with_more_than_32_series_slots(G, variant, mode, engines, oracle_c, oracle_np, plan_exe, sm_count):
     """ADVICE r1: a pod may carry more than 32 series (duplicate exporters, a pod name reused across hosts): the
-    per-pod flag mask is ceil(G / 32) words; verdicts, counts and the power veto equal the oracle's"""
+    per-pod flag mask is ceil(G / 32) words; verdicts, counts, every row's idle slot and the power veto equal the
+    oracle's"""
     eng = engines[variant]
     rng = np.random.default_rng(G)
     P, T = 70, 24
@@ -496,13 +607,17 @@ def test_pods_with_more_than_32_series_slots(G, variant, engines, oracle_c):
     w[7, G - 1, 3] = 400.0                                  # the veto too
     e = (rng.random(P) < 0.9).astype(np.uint8)
     for thr in (0.0, 150.0):
-        d = eng.decide(u, w, e, power_threshold=thr, want_series_max=True)
+        assert_ran(plan_exe, sm_count, variant, mode, T, P * G * (2 if thr else 1))
+        d = eng.decide(u, w, e, power_threshold=thr, want_series_max=mode == "whole", want_veto=True,
+                       want_idle_slots=mode == "early")
         exp = oracle_c.decide(u, w, e, power_threshold=thr)
-        _check(d.decision_bits, d.candidate_bits, (d.n_series, d.n_candidates, d.n_decisions), exp, d.series_max)
+        _check(d.decision_bits, d.candidate_bits, (d.n_series, d.n_candidates, d.n_decisions), exp, d.series_max,
+               d.idle_slots)
+        assert np.array_equal(d.veto_bits, oracle_np.decide(u, w, e, power_threshold=thr)["veto_bits"])
     # device-resident window through the same kernels
-    bits, cbits, counts, smax, _ = _device_decide(eng, u)
+    bits, cbits, counts, smax, _, islots = _device_decide(eng, u, **_outputs(mode))
     exp0 = oracle_c.decide(u)
-    _check(bits, cbits, counts, exp0, smax)
+    _check(bits, cbits, counts, exp0, smax, islots)
 
 
 def test_memory_and_timing_helpers(engines):

@@ -2,17 +2,24 @@
 the windows of tests/test_probe_emul.py (a settling sample at every head and chunk boundary, and the f32 edge values)
 from dense, strided, host (staged) and resident-ring memory, with the power plane on and off; a PDL batch in which
 early-exit calls alternate with series_max calls, so the probe kernel and k_reduce_tma follow each other with different
-shared-memory footprints; and the C2- and C3-shaped synthetic windows, all against the oracles."""
+shared-memory footprints; the C2- and C3-shaped synthetic windows; and every ring layout the kernel can take, all
+against the oracles."""
 import numpy as np
 import pytest
 import torch
 
+import geometry
 import test_early_exit_emul as EE
 import test_probe_emul as PE
 from test_gpu_geometry import DEV, _check, _device_decide, _oracle_synth, _synth, _u32
 
 pytestmark = pytest.mark.gpu
 THR = PE.THR
+
+
+@pytest.fixture(scope="module")
+def plan_exe(tmp_path_factory):
+    return geometry.build(tmp_path_factory.mktemp("launch_plan"))
 
 
 def _windows():
@@ -42,7 +49,7 @@ def test_boundary_and_edge_windows(oracle_np):
                         wrows = np.full((P * G, ld), 1e9, np.float32)
                         wrows[:, :T] = power.reshape(P * G, T)
                         w_t = torch.from_numpy(wrows).to(DEV)
-                    bits, cbits, counts, _, vb = _device_decide(
+                    bits, cbits, counts, _, vb, _ = _device_decide(
                         eng, u_t.data_ptr(), P, G, T, w_t.data_ptr() if use_power else None, {}, thr,
                         stride=stride, want_smax=False, want_veto=True)
                     _check(bits, cbits, counts, exp, None, vb if use_power else None)
@@ -126,7 +133,91 @@ def test_synthetic_windows_equal_the_c_oracle(shape, oracle_c):
             u, w, e = _synth(eng, 0x5EED0002, P, G, T, power)
             exp = _oracle_synth(oracle_c, 0x5EED0002, P, G, T, power, smax=False)
             for rep in range(2):
-                bits, cbits, counts, _, vb = _device_decide(
+                bits, cbits, counts, _, vb, _ = _device_decide(
                     eng, u, P, G, T, w, {"eligible": e.cpu().numpy()}, 150.0 if power else 0.0, want_smax=False,
                     want_veto=power)
                 _check(bits, cbits, counts, exp, None, vb if power else None)
+
+
+def _ring_layouts(plan_exe, sm_count):
+    """(stage_bytes, depth) -> the window lengths T = 4 .. 7200 (multiples of 4) whose probe ring has that layout"""
+    Ts = list(range(4, 7201, 4))
+    knobs = geometry.Knobs(sm_count=sm_count)
+    out = {}
+    for T, p in zip(Ts, geometry.plans(plan_exe, [(knobs, "auto", T, 1 << 20, True, False, 1, True) for T in Ts])):
+        assert p.kernel == "probe", p
+        out.setdefault((p.stage_bytes, p.depth), []).append(T)
+    return out
+
+
+def _base_rows(T, power, rng):
+    """the rows a window is drawn from: a settling sample at every head and chunk boundary (one row each, and one
+    that nothing settles), idle rows, and rows with gaps of no sample; -> (rows, how often each is drawn)"""
+    quiet = 100.0 if power else 0.0
+    boundary = PE._boundary_window(T, power).reshape(-1, T)
+    idle = np.full((4, T), quiet, np.float32)
+    gapped = np.full((8, T), quiet, np.float32)
+    for r in range(gapped.shape[0]):
+        for _ in range(3):
+            a = int(rng.integers(0, T))
+            gapped[r, a:a + int(rng.integers(1, max(2, T // 4)))] = np.nan
+    gapped[-1] = np.nan                               # no sample at all: never idle, never vetoes
+    rows = np.concatenate([boundary, idle, gapped])
+    share = (0.2, 0.7) if power else (0.4, 0.3)         # (boundary, idle): the rest have gaps
+    p = np.concatenate([np.full(len(boundary), share[0] / len(boundary)), np.full(len(idle), share[1] / len(idle)),
+                        np.full(len(gapped), (1 - sum(share)) / len(gapped))])
+    return rows, p
+
+
+def _pack(flags):
+    b = np.zeros((len(flags) + 31) // 32 * 32, bool)
+    b[:len(flags)] = flags
+    return np.packbits(b, bitorder="little").view("<u4")
+
+
+def test_every_ring_layout(plan_exe, oracle_c):
+    """each of the probe kernel's ring layouts (stage size and depth, gpr_launch.h probe_layout) at the shortest and
+    the longest window that takes it: enough rows that every warp of every CTA refills its ring several times, and a
+    single series (P = G = 1, fewer rows than one CTA has stages); util alone and util + power, with gates; the bitmaps,
+    counts, veto bits and every row's idle slot against the oracle"""
+    import gpu_pruner_b200 as g
+    with g.IdleEngine(device=0) as eng:
+        sm_count = eng.device_info()["sm_count"]
+        layouts = _ring_layouts(plan_exe, sm_count)
+        assert len(layouts) == 16 and {d for _, d in layouts} >= {3, 32}
+        for (stage_bytes, depth), Ts in sorted(layouts.items()):
+            for T in sorted({Ts[0], Ts[-1]}):
+                rng = np.random.default_rng(T)
+                for use_power in (False, True):
+                    planes = 2 if use_power else 1
+                    for many in (True, False):
+                        G = 4 if many else 1
+                        # 4 rows per warp stage: each ring is refilled with new rows at least 3 times
+                        P = -(-4 * sm_count * 32 * depth // (planes * G)) if many else 1
+                        rows, pr = _base_rows(T, False, rng)
+                        u = rows[rng.choice(len(rows), P * G, p=pr)].reshape(P, G, T)
+                        w = None
+                        if use_power:
+                            rows, pr = _base_rows(T, True, rng)
+                            w = rows[rng.choice(len(rows), P * G, p=pr)].reshape(P, G, T)
+                        kw = {"eligible": (rng.random(P) < 0.9).astype(np.uint8),
+                              "created_ts": rng.integers(1000, 2000, P).astype(np.int64), "cutoff_ts": 1500}
+                        thr = THR if use_power else 0.0
+                        tag = (T, stage_bytes, depth, use_power, P, G)
+                        p = geometry.plan(plan_exe, geometry.Knobs(sm_count=sm_count), "auto", T, P * G * planes,
+                                          True, False, P, True)
+                        assert p.kernel == "probe" and (p.stage_bytes, p.depth) == (stage_bytes, depth), (tag, p)
+                        assert p.grid == (sm_count if many else 1), (tag, p)
+                        assert (P * G * planes >= 3 * p.grid * 32 * depth) if many else (P * G * planes < 32 * depth)
+                        exp = oracle_c.decide(u, w, kw["eligible"], kw["created_ts"], kw["cutoff_ts"], thr,
+                                              n_threads=8)
+                        exp["veto_bits"] = _pack(np.any(w.astype(np.float64) >= THR, axis=(1, 2)) if use_power
+                                                 else np.zeros(P, bool))
+                        assert 0 < exp["n_candidates"] < P or not many, tag
+                        u_t = torch.from_numpy(u).to(DEV)
+                        w_t = torch.from_numpy(w).to(DEV) if use_power else None
+                        bits, cbits, counts, _, vb, isl = _device_decide(eng, u_t, P, G, T, w_t, kw, thr,
+                                                                          want_smax=False, want_veto=True,
+                                                                          want_slots=True)
+                        _check(bits, cbits, counts, exp, None, vb, isl)
+                        del u_t, w_t

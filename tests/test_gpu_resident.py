@@ -1,12 +1,14 @@
 """The resident ring of daemon mode through libgpr.so on an H100, against the numpy ring model of
 tests/ring_scripts.py and the float64 oracle.
 
-Every script of tests/test_ring_emul.py runs on two engines per kernel variant (GPR_KERNEL=ldg / tma): one whose ring
-keeps the block index (GPR_F_BLOCK_INDEX, deciding on idx_ld = ceil(T / 64) padded to a multiple of 4 "samples" per
-series, a TMA-able row) and one that rescans the ring.  After every operation the ring is read back and must equal the
-model bit for bit, and gpr_decide_resident (power threshold 150 W) must give the oracle's verdict on the unrolled
-window; the two engines must agree.  The appended columns come from pageable and pinned host memory and from device
-memory, at a 16-byte and at a 4-byte aligned address."""
+Every script of tests/test_ring_emul.py runs on two engines per kernel variant (GPR_KERNEL=ldg / tma / auto): one whose
+ring keeps the block index (GPR_F_BLOCK_INDEX, deciding on idx_ld = ceil(T / 64) padded to a multiple of 4 "samples"
+per series, a TMA-able row) and one that rescans the ring.  After every operation the ring is read back and must equal
+the model bit for bit, and gpr_decide_resident (power threshold 150 W) must give the oracle's verdict on the unrolled
+window twice: once with series_max (every row read whole) and once with idle_slots and no series_max (rows stop at
+their first settling sample; AUTO runs the probe kernel), every row's idle slot checked; the two engines must agree.
+The appended columns come from pageable and pinned host memory and from device memory, at a 16-byte and at a 4-byte
+aligned address."""
 import json
 
 import numpy as np
@@ -14,11 +16,12 @@ import pytest
 
 import kat
 import ring_scripts as RS
+from test_gpu_parity import assert_ran, expected_idle_slots, plan_exe, resident_ld  # noqa: F401 (a fixture)
 
 pytestmark = pytest.mark.gpu
 
 torch = pytest.importorskip("torch")
-VARIANTS = ["ldg", "tma"]
+VARIANTS = ["ldg", "tma", "auto"]
 CASES = RS.cases()
 SOURCES = ["pageable", "pinned", "device", "device+4"]
 _MAX_CELLS = 1 << 20    # the largest source of any script: rows * ld per plane
@@ -54,28 +57,40 @@ def expected(m: RS.Ring):
     return exp
 
 
-def decide(eng, m: RS.Ring):
+def decide(eng, m: RS.Ring, early=False):
+    """gpr_decide_resident with series_max, or (early) with idle_slots and no series_max"""
     from gpu_pruner_b200 import ffi
     W = max((m.P + 31) // 32, 1)
     db, cb, vb = (np.full(W, 0xDEADBEEF, np.uint32) for _ in range(3))
-    sm = np.full((m.P, m.G), -777.0, np.float32)
-    r = eng.decide_ptr(None, 0, 0, 0, db, candidate_bits=cb, series_max=sm, veto_bits=vb,
+    sm = None if early else np.full((m.P, m.G), -777.0, np.float32)
+    isl = np.full((max(m.P, 1), (m.G + 31) // 32), 0xDEADBEEF, np.uint32) if early else None
+    r = eng.decide_ptr(None, 0, 0, 0, db, candidate_bits=cb, series_max=sm, veto_bits=vb, idle_slots=isl,
                        power_threshold=RS.THR if len(m.planes) > 1 else 0.0, in_kind=ffi.GPR_MEM_HOST,
                        out_kind=ffi.GPR_MEM_HOST, resident=True)
     W = (m.P + 31) // 32
-    return {"decision_bits": db[:W], "candidate_bits": cb[:W], "veto_bits": vb[:W], "series_max": sm,
-            "n_series": r.n_series, "n_candidates": r.n_candidates, "n_decisions": r.n_decisions}
+    out = {"decision_bits": db[:W], "candidate_bits": cb[:W], "veto_bits": vb[:W],
+           "n_series": r.n_series, "n_candidates": r.n_candidates, "n_decisions": r.n_decisions}
+    if early:
+        out["idle_slots"] = isl[:m.P]
+    else:
+        out["series_max"] = sm
+    return out
 
 
 def same_verdict(got, exp):
+    """None, or the first output of `got` that differs from `exp` (an oracle result or another engine's)"""
     for k in ("decision_bits", "candidate_bits", "veto_bits"):
         if not np.array_equal(got[k], exp[k]):
             return k
     if (got["n_series"], got["n_candidates"], got["n_decisions"]) != \
             (exp["n_series"], exp["n_candidates"], exp["n_decisions"]):
         return "counts"
-    if not kat.smax_equal(got["series_max"], exp["series_max"]):
+    if "series_max" in got and not kat.smax_equal(got["series_max"], exp["series_max"]):
         return "series_max"
+    if "idle_slots" in got:
+        want = exp["idle_slots"] if "idle_slots" in exp else expected_idle_slots(exp["series_max"])
+        if not np.array_equal(got["idle_slots"], want):
+            return "idle_slots"
     return None
 
 
@@ -155,23 +170,32 @@ def run_script(eng, bufs, case, index):
         if op[0] == "write" and index and not (last_write and not case.flags & 2):
             out.append(None)                # the index is rebuilt by the reindex that follows (gpr.h)
             continue
-        got = decide(eng, m)
-        bad = same_verdict(got, expected(m))
-        assert bad is None, f"{case.name} op {i} ({op[0]} {op[1:2]}), index={index}: {bad} differs from the oracle"
+        exp = expected(m)
+        got = [decide(eng, m), decide(eng, m, early=True)]
+        for g, mode in zip(got, ("whole", "early")):
+            bad = same_verdict(g, exp)
+            assert bad is None, \
+                f"{case.name} op {i} ({op[0]} {op[1:2]}), index={index}, {mode}: {bad} differs from the oracle"
         out.append(got)
     return out
 
 
 @pytest.mark.parametrize("variant", VARIANTS)
 @pytest.mark.parametrize("case", CASES, ids=[c.name for c in CASES])
-def test_ring_scripts(case, variant, engines):
+def test_ring_scripts(case, variant, engines, plan_exe):
     e, bufs = engines
+    sm_count = e[(variant, True)].device_info()["sm_count"]
+    for index in (True, False):
+        for mode in ("whole", "early"):
+            assert_ran(plan_exe, sm_count, variant, mode, resident_ld(case.T, index),
+                       case.P * case.G * (2 if case.flags & 1 else 1), resident_ld(case.T, index) % 4 == 0)
     a = run_script(e[(variant, True)], bufs[(variant, True)], case, True)
     b = run_script(e[(variant, False)], bufs[(variant, False)], case, False)
     assert len(a) == len(b) == len(case.ops)
     for i, (x, y) in enumerate(zip(a, b)):
         if x is not None:
-            assert same_verdict(x, y) is None, (case.name, i)
+            for mode, xm, ym in zip(("whole", "early"), x, y):
+                assert same_verdict(xm, ym) is None, (case.name, i, mode)
 
 
 @pytest.mark.parametrize("index", [False, True], ids=["rescan", "block-index"])
