@@ -8,28 +8,22 @@ import math
 import os
 import random
 import struct
-import subprocess
 
 import numpy as np
 import pytest
+
+import numbers_corpus as NC
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
 def driver(tmp_path_factory):
-    out = tmp_path_factory.mktemp("num") / "number_check"
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-fsanitize=undefined", "-fno-sanitize-recover=all",
-                           os.path.join(ROOT, "tests", "cpp", "number_check.cpp"), "-o", str(out)])
-    return str(out)
+    return NC.build_number_check(tmp_path_factory.mktemp("num") / "number_check")
 
 
 def _run(driver, lines):
-    r = subprocess.run([driver], input="\n".join(lines) + "\n", capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0, r.stderr[-2000:]
-    out = r.stdout.splitlines()
-    assert len(out) == len(lines)
-    return out
+    return NC.run_number_check(driver, lines)
 
 
 def _bits64(x):
@@ -50,31 +44,7 @@ def test_pow10_table_is_what_the_generator_writes():
 
 
 def test_eisel_lemire_matches_correct_rounding(driver):
-    rng = random.Random(20260921)
-    cases = []
-    realistic = set()
-    for _ in range(120_000):
-        nd = rng.randrange(1, 20)
-        man = rng.randrange(10 ** (nd - 1), 10 ** nd)
-        if man >= 1 << 64:
-            continue
-        cases.append((man, rng.randrange(-340, 300)))
-    # shortest-round-trip representations of random doubles (what Prometheus prints), as mantissa / exponent
-    for _ in range(80_000):
-        x = rng.random() if rng.random() < 0.7 else rng.uniform(0, 1000)
-        s = repr(x)
-        if "e" in s or "." not in s:
-            continue
-        ip, fp = s.split(".")
-        cases.append((int(ip + fp), -len(fp)))
-        realistic.add(cases[-1])
-    # numbers at and around rounding boundaries
-    for k in (53, 54, 60, 63):
-        for d in (-1, 0, 1):
-            cases.append(((1 << k) + d, 0))
-            cases.append(((1 << k) + d, -5))
-    cases += [(9007199254740993, 0), (9007199254740993, -3), (1, -324), (1, 308), (17976931348623157, 292),
-              (22250738585072014, -324), (4, -324), (12345678901234567890, 0), (1, 0), (5, -1)]
+    cases, realistic = NC.eisel_lemire_cases()
     out = _run(driver, [f"E {m} {e}" for m, e in cases])
     declined = 0
     for (m, e), line in zip(cases, out):
@@ -89,22 +59,7 @@ def test_eisel_lemire_matches_correct_rounding(driver):
 
 
 def test_parse_value_matches_strtod_then_float(driver):
-    rng = random.Random(7)
-    texts = ["0", "-0", "100", "37", "0.5", "0.25", "12.25", "0.30000000000000004", "123456789012345678",
-             "0.1", "0.07", "99.99999999999999", "1234567.1234567", "16777216", "16777217", "4294967296.5",
-             "0.000000000000000000000000000000000000000000001", "0.0000000000000000000000000000000000000000000001",
-             "340282350000000000000000000000000000000", "0.1234567890123456789", "1.7976931348623157",
-             "000123", "0.000", "5.0000000000000000000", "5e-07", "1.2345e+21", "1e2", "1E1", "1e-50", "1e23",
-             "9.999999e-07", "1e+21", "0e0", "3.4028235e+38", "1e39", "4.9e-324", "1.5e-46"]
-    for _ in range(60_000):
-        x = rng.random() if rng.random() < 0.6 else rng.uniform(0, 700)
-        texts.append(repr(x))          # includes Go-style exponent forms for the tiny ones ("5e-07")
-        if rng.random() < 0.05:
-            texts.append(repr(x * 10.0 ** rng.randrange(-30, 30)))
-        if rng.random() < 0.1:
-            texts.append(str(rng.randrange(0, 101)))
-        if rng.random() < 0.05:
-            texts.append("-" + texts[-1])
+    texts = NC.value_texts()
     out = _run(driver, ["V " + t for t in texts])
     declined = []
     for t, line in zip(texts, out):
