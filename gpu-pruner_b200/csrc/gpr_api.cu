@@ -1188,11 +1188,9 @@ int gpr_sync(gpr_ctx* ctx) {
 static int decide_blocking(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resident) {
   int rc = decide_impl(ctx, win, res, resident, false);
   if (rc != GPR_OK) {
-    if (ctx) {
-      cudaStreamSynchronize(ctx->stream);
-      ctx->pending.clear();
-      ctx->masks_dirty = true;
-    }
+    // like the async paths: decisions enqueued before this call stay pending, and the next gpr_sync or
+    // successful blocking call fills their counters; this call enqueued no result of its own
+    if (ctx) ctx->masks_dirty = true;
     return rc;
   }
   rc = sync_impl(ctx);

@@ -230,10 +230,14 @@ GPR_API void gpr_destroy(gpr_ctx *ctx);
 GPR_API const char *gpr_last_error(const gpr_ctx *ctx);
 
 /* ---- the hot path -------------------------------------------------------------------- */
-/* Blocking: on return the result buffers and counters are complete.                      */
+/* Blocking: on return the result buffers and counters are complete, and so are those of every
+ * decision enqueued before it (the call retires them like gpr_sync).  A failing call never drops
+ * or changes decisions enqueued before it: they stay pending for the next gpr_sync.       */
 GPR_API int gpr_decide(gpr_ctx *ctx, const gpr_window *win, gpr_result *res);
 /* Enqueue only (device or pinned-host buffers); counters are filled by gpr_sync().       */
 GPR_API int gpr_decide_async(gpr_ctx *ctx, const gpr_window *win, gpr_result *res);
+/* Waits for everything enqueued and fills the counters of every pending result, whatever failed in
+ * between (a failed gpr_decide / gpr_decide_resident / _async call leaves earlier results pending). */
 GPR_API int gpr_sync(gpr_ctx *ctx);
 /* Enqueue n independent decisions (windows[i] -> results[i]) in one call: the same as n calls of
  * gpr_decide_async, without n trips through the caller's FFI.  At most 256 results may be

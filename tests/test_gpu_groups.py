@@ -20,12 +20,32 @@ pytestmark = pytest.mark.gpu
 THR = GE.THR
 
 
+CHUNK_PODS = 24   # pods per 1 MB staging chunk of a 3 x 1800 window with power (48 without)
+
+
+def _chunked_window():
+    """150 x 3 x 1800: 7 staging chunks with power and 4 without at GPR_CHUNK_MB=1, and a table that changes from
+    chunk to chunk (no groups; all three slots one group; slots 1-2 one group), so a chunk that read another chunk's
+    grouped rows or wrote its row maxima over another chunk's would decide differently"""
+    rng = np.random.default_rng(77)
+    P, G, T = 150, 3, 1800
+    layouts = [[0, 1, 2], [0, 0, 0], [0, 1, 1]]
+    table = np.array([layouts[(p // CHUNK_PODS) % 3] for p in range(P)], np.uint32)
+    table |= np.where(rng.random((P, G)) < 0.5, R.UTIL, 0).astype(np.uint32)
+    m = np.array(R.PALETTE, np.float32)[rng.integers(0, len(R.PALETTE), (P, G))]
+    util = R.window_for(rng, m, T)
+    power = np.full((P, G, T), 100.0, np.float32)
+    power[rng.random(P) < 0.2, 0, T // 3] = THR
+    return util, power, table
+
+
 def _cases():
     out = []
     for i, (P, G, T, size) in enumerate(GE.SHAPES):
         out.append((f"gen{i}", *GE._generated(100 + i, P, G, T, max_size=size)))
     u, table, _ = GE._host_window()
     out.append(("ingested", u, None, table))
+    out.append(("chunked", *_chunked_window()))
     return out
 
 
@@ -79,8 +99,15 @@ def _device(eng, util, power, table, use_power, smax, stride=0, offset=0, u8=Fal
 
 @pytest.mark.parametrize("kernel", ["ldg", "tma"])
 def test_windows_from_every_source(kernel):
+    """device windows (dense, strided, misaligned) and host windows, the host ones also staged in 1 MB chunks
+    (GPR_CHUNK_MB=1), where the windows of 1800 samples span several chunks and the table follows them"""
     import gpu_pruner_b200 as g
-    with g.IdleEngine(device=0, kernel=kernel, max_pods=128, max_gpus=256, max_samples=2048, power_plane=True) as eng:
+    from test_gpu_geometry import _environ
+    caps = dict(device=0, kernel=kernel, max_pods=256, max_gpus=256, max_samples=2048, power_plane=True)
+    with _environ({"GPR_CHUNK_MB": "1"}):
+        chunked = g.IdleEngine(**caps)
+    with g.IdleEngine(**caps) as eng, chunked:
+        assert 150 * 3 * 1800 * 8 > 6 << 20      # the chunked case: more than six 1 MB chunks with power
         for name, util, power, table in _cases():
             P, G, T = util.shape
             for use_power in (False, True) if power is not None else (False,):
@@ -98,10 +125,15 @@ def test_windows_from_every_source(kernel):
                                 assert np.array_equal(np.isnan(sm), np.isnan(m)) and np.array_equal(
                                     np.nan_to_num(sm), np.nan_to_num(m)), tag
                                 smax_by_table.setdefault(t is not None, sm)
-                        d = eng.decide(util, power if use_power else None, power_threshold=THR if use_power else 0.0,
-                                       want_series_max=smax, groups=t, want_idle_slots=True)
-                        _check((d.decision_bits, d.candidate_bits, (d.n_series, d.n_candidates, d.n_decisions),
-                                d.idle_slots), w, (kernel, name, "host", use_power, smax, t is not None))
+                        for e, leg in ((eng, "host"), (chunked, "host, 1 MB chunks")):
+                            d = e.decide(util, power if use_power else None, power_threshold=THR if use_power else 0.0,
+                                         want_series_max=smax, groups=t, want_idle_slots=True)
+                            _check((d.decision_bits, d.candidate_bits, (d.n_series, d.n_candidates, d.n_decisions),
+                                    d.idle_slots), w, (kernel, name, leg, use_power, smax, t is not None))
+                            if smax:
+                                m = R.row_max(util)
+                                assert np.array_equal(np.isnan(d.series_max), np.isnan(m)) and np.array_equal(
+                                    np.nan_to_num(d.series_max), np.nan_to_num(m)), (kernel, name, leg)
                     if smax:   # series_max does not depend on the table
                         assert _smax_equal(smax_by_table[True], smax_by_table[False]), (kernel, name)
 
