@@ -200,13 +200,16 @@ struct gpr_ctx {
   // chunk size.  Pageable text: GPR_TEXT_CHUNK_MB (1..16), default 2 — the pinned staging ring is
   // up_threads x 2 x chunk, and page-locking it is paid by the first scan of a process, so a small chunk keeps
   // that set-up cheap.  Pinned / device text needs no staging and goes in 16 MB pieces.
+  // Whatever the chunk, its markers are collected per scan unit of at most kScanUnit bytes, one marker block
+  // each: the room per byte of text is the same for every source and chunk size.
   static constexpr size_t kPinnedChunk = 16u << 20;
-  static constexpr int kMarkBlocks = 64;                   // ring of marker blocks (chunks in flight ahead of the consumer)
-  static constexpr uint32_t kMarkCap = 16384;              // markers of one kind per chunk (2 MB: one per 128 B)
+  static constexpr size_t kScanUnit = 2u << 20;
+  static constexpr int kMarkBlocks = 64;                   // ring of marker blocks (units in flight ahead of the consumer)
+  static constexpr uint32_t kMarkCap = 16384;              // markers of one kind per unit (2 MB: one per 128 B)
   size_t up_chunk = 2u << 20;
   size_t up_slot_bytes = 0;            // up_chunk + a page (the 16 bytes of overlap, page aligned)
   unsigned char* h_up_ring = nullptr;  // [up_threads][kUpSlots][up_slot_bytes], pinned
-  uint32_t* h_mark_blocks = nullptr;   // [kMarkBlocks][2 + 2 * kMarkCap], pinned + device-mapped
+  uint32_t* h_mark_blocks = nullptr;   // [kMarkBlocks][2 + 2 * kMarkCap], pinned + device-mapped (8 MB)
   uint32_t* d_mark_blocks = nullptr;   // the same in device memory: the scan appends here (atomics), then publishes
   cudaStream_t up_stream[kUpThreads] = {};
   cudaEvent_t up_event[kUpThreads][kUpSlots] = {};
@@ -830,45 +833,53 @@ int sync_impl(gpr_ctx* ctx) {
 // double buffer (pageable sources; a plain cudaMemcpy would go through the driver's single bounce buffer at
 // ~10 GB/s), enqueue the H2D copy on their own stream, and right behind it the scan kernel for that chunk, which
 // appends the chunk's markers to a block of mapped pinned memory.  A chunk is copied with 16 bytes of overlap
-// into the next one (identical bytes written twice), so its scan never needs another stream's data.  The
-// consumer (gpr_text_scan_next) takes the chunks in text order while later ones are still in flight.
+// into the next one (identical bytes written twice), so its scan never needs another stream's data.  A chunk
+// is cut into scan units of at most kScanUnit bytes (unit j of chunk c is [c * chunk + j * unit, ...), global
+// index c * units_per_chunk + j), and each unit's markers go to a block of their own.  The consumer
+// (gpr_text_scan_next) takes the units in text order while later chunks are still in flight.
 struct ScanPipe {
   int slot = 0;
   const char* src = nullptr;
   uint8_t* dst = nullptr;
   uint64_t n = 0, n_chunks = 0, chunk = 0;
+  uint64_t unit = 0, units_per_chunk = 1, n_units = 0;
   int nt = 1;
   int src_kind = GPR_MEM_HOST;
   bool staged = false;  // source is pageable host memory: goes through the pinned ring
   std::vector<std::thread> th;
-  std::atomic<uint64_t> consumed{0};                      // chunks handed to the caller
-  std::atomic<uint64_t> recorded[gpr_ctx::kMarkBlocks];   // chunk + 1 whose event has been recorded in this block
+  std::atomic<uint64_t> consumed{0};                      // units handed to the caller
+  std::atomic<uint64_t> recorded[gpr_ctx::kMarkBlocks];   // unit + 1 whose event has been recorded in this block
   std::atomic<int> error{0};                              // first cudaError_t of a producer
   std::atomic<bool> stop{false};
-  uint64_t next = 0;                                      // next chunk the consumer returns
+  uint64_t next = 0;                                      // next unit the consumer returns
 };
 
 namespace {
 
 constexpr uint32_t kBlockWords = 2 + 2 * gpr_ctx::kMarkCap;
 
-// markers of one chunk, 32-bit offsets relative to the chunk: [n_open, n_close, opens[cap], closes[cap]]
+// markers of one chunk, each in the block of its unit, as 32-bit offsets relative to the unit:
+// [n_open, n_close, opens[cap], closes[cap]] per block; the chunk's first unit has global index u0
 struct ChunkSink {
-  uint32_t* block;
-  uint64_t base;
-  __device__ __forceinline__ void values_open(uint64_t p) {
-    const uint32_t i = atomicAdd(block + 0, 1u);
-    if (i < gpr_ctx::kMarkCap) block[2 + i] = (uint32_t)(p - base);
+  uint32_t* blocks;  // the device ring, kMarkBlocks blocks
+  uint64_t base, unit, u0;
+  __device__ __forceinline__ void put(uint64_t p, uint32_t which) {
+    const uint64_t j = (p - base) / unit;
+    uint32_t* block = blocks + (size_t)((u0 + j) % gpr_ctx::kMarkBlocks) * kBlockWords;
+    const uint32_t i = atomicAdd(block + which, 1u);
+    if (i < gpr_ctx::kMarkCap) block[2 + which * gpr_ctx::kMarkCap + i] = (uint32_t)(p - base - j * unit);
   }
-  __device__ __forceinline__ void values_close(uint64_t p) {
-    const uint32_t i = atomicAdd(block + 1, 1u);
-    if (i < gpr_ctx::kMarkCap) block[2 + gpr_ctx::kMarkCap + i] = (uint32_t)(p - base);
-  }
+  __device__ __forceinline__ void values_open(uint64_t p) { put(p, 0); }
+  __device__ __forceinline__ void values_close(uint64_t p) { put(p, 1); }
 };
 
-// copies a chunk's markers from the device block to the host-mapped one with plain coalesced stores (the scan's
-// atomic appends must not go to host memory: an atomic across PCIe costs microseconds)
-__global__ void __launch_bounds__(256) k_publish_marks(const uint32_t* __restrict__ d_block, uint32_t* __restrict__ h_block) {
+// copies the markers of units u0 .. u0 + gridDim.x - 1 from their device blocks to the host-mapped ones with plain
+// coalesced stores (the scan's atomic appends must not go to host memory: an atomic across PCIe costs microseconds)
+__global__ void __launch_bounds__(256) k_publish_marks(const uint32_t* __restrict__ d_blocks, uint32_t* __restrict__ h_blocks,
+                                                       uint64_t u0) {
+  const size_t at = (size_t)((u0 + blockIdx.x) % gpr_ctx::kMarkBlocks) * kBlockWords;
+  const uint32_t* d_block = d_blocks + at;
+  uint32_t* h_block = h_blocks + at;
   const uint32_t no = min(d_block[0], gpr_ctx::kMarkCap), nc = min(d_block[1], gpr_ctx::kMarkCap);
   for (uint32_t i = threadIdx.x; i < no; i += blockDim.x) h_block[2 + i] = d_block[2 + i];
   for (uint32_t i = threadIdx.x; i < nc; i += blockDim.x)
@@ -877,8 +888,8 @@ __global__ void __launch_bounds__(256) k_publish_marks(const uint32_t* __restric
 }
 
 __global__ void __launch_bounds__(256) k_text_scan_chunk(const uint8_t* __restrict__ t, uint64_t n, uint64_t slice_begin,
-                                                         uint64_t slice_end, uint32_t* block) {
-  ChunkSink sink{block, slice_begin * gpr::text::kScanBytes};
+                                                         uint64_t slice_end, uint32_t* blocks, uint64_t unit, uint64_t u0) {
+  ChunkSink sink{blocks, slice_begin * gpr::text::kScanBytes, unit, u0};
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   for (uint64_t slice = slice_begin + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; slice < slice_end; slice += stride)
     gpr::text::scan_slice(t, n, slice, sink);
@@ -892,15 +903,16 @@ void scan_producer(gpr_ctx* ctx, ScanPipe* sp, int k) {
   int slot = 0;
   cudaStream_t st = ctx->up_stream[k];
   for (uint64_t c = (uint64_t)k; c < sp->n_chunks && e == cudaSuccess && !sp->stop.load(); c += (uint64_t)sp->nt) {
-    // the marker block of this chunk is free once the consumer has taken chunk c - NB
-    for (int spins = 0; c >= sp->consumed.load(std::memory_order_acquire) + NB && !sp->stop.load(); ++spins) {
+    const uint64_t off = c * sp->chunk;
+    const uint64_t len = std::min<uint64_t>(sp->chunk, sp->n - off);
+    const uint64_t len_ov = std::min<uint64_t>(len + 16, sp->n - off);  // overlap into the next chunk
+    const uint64_t u0 = c * sp->units_per_chunk, nu = (len + sp->unit - 1) / sp->unit;
+    // the marker block of unit u is free once the consumer has taken unit u - NB (NB >= units_per_chunk)
+    for (int spins = 0; u0 + nu > sp->consumed.load(std::memory_order_acquire) + NB && !sp->stop.load(); ++spins) {
       if (spins < 64) std::this_thread::yield();
       else std::this_thread::sleep_for(std::chrono::microseconds(50));  // a slow consumer: do not burn the core
     }
     if (sp->stop.load()) break;
-    const uint64_t off = c * sp->chunk;
-    const uint64_t len = std::min<uint64_t>(sp->chunk, sp->n - off);
-    const uint64_t len_ov = std::min<uint64_t>(len + 16, sp->n - off);  // overlap into the next chunk
     const void* from = sp->src + off;
     if (sp->staged) {
       unsigned char* buf = ctx->h_up_ring + ((size_t)k * NS + slot) * SLOT;
@@ -914,20 +926,20 @@ void scan_producer(gpr_ctx* ctx, ScanPipe* sp, int k) {
     if (e == cudaSuccess && sp->staged) e = cudaEventRecord(ctx->up_event[k][slot], st), used[slot] = true;
     slot = (slot + 1) % NS;
     if (e != cudaSuccess) break;
-    // (the kernels that last used block c % NB have completed: their chunk was consumed)
-    uint32_t* h_block = ctx->h_mark_blocks + (size_t)(c % NB) * kBlockWords;
-    uint32_t* d_block = ctx->d_mark_blocks + (size_t)(c % NB) * kBlockWords;
-    e = cudaMemsetAsync(d_block, 0, 2 * sizeof(uint32_t), st);
+    // (the kernels that last used the blocks of units u0 .. u0 + nu - 1 have completed: their units were consumed)
+    for (uint64_t u = u0; u < u0 + nu && e == cudaSuccess; ++u)
+      e = cudaMemsetAsync(ctx->d_mark_blocks + (size_t)(u % NB) * kBlockWords, 0, 2 * sizeof(uint32_t), st);
     if (e != cudaSuccess) break;
     const uint64_t s0 = off / gpr::text::kScanBytes;
     const uint64_t s1 = (off + len + gpr::text::kScanBytes - 1) / gpr::text::kScanBytes;
     const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((s1 - s0 + 255) / 256, (uint64_t)ctx->sm_count * 8));
-    k_text_scan_chunk<<<grid, 256, 0, st>>>(sp->dst, sp->n, s0, s1, d_block);
-    k_publish_marks<<<1, 256, 0, st>>>(d_block, h_block);
+    k_text_scan_chunk<<<grid, 256, 0, st>>>(sp->dst, sp->n, s0, s1, ctx->d_mark_blocks, sp->unit, u0);
+    k_publish_marks<<<(uint32_t)nu, 256, 0, st>>>(ctx->d_mark_blocks, ctx->h_mark_blocks, u0);
     e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaEventRecord(ctx->mark_event[c % NB], st);
-    if (e != cudaSuccess) break;
-    sp->recorded[c % NB].store(c + 1, std::memory_order_release);
+    for (uint64_t u = u0; u < u0 + nu && e == cudaSuccess; ++u) {
+      e = cudaEventRecord(ctx->mark_event[u % NB], st);
+      if (e == cudaSuccess) sp->recorded[u % NB].store(u + 1, std::memory_order_release);
+    }
   }
   if (e != cudaSuccess) {
     int zero = 0;
@@ -1662,6 +1674,12 @@ int gpr_text_scan_begin(gpr_ctx* ctx, int32_t slot, const char* text, uint64_t n
   }
   sp->chunk = sp->staged ? ctx->up_chunk : gpr_ctx::kPinnedChunk;
   sp->n_chunks = (n_bytes + sp->chunk - 1) / sp->chunk;
+  sp->unit = std::min<uint64_t>(sp->chunk, gpr_ctx::kScanUnit);
+  sp->units_per_chunk = (sp->chunk + sp->unit - 1) / sp->unit;
+  sp->n_units = sp->n_chunks ? (sp->n_chunks - 1) * sp->units_per_chunk +
+                                   (n_bytes - (sp->n_chunks - 1) * sp->chunk + sp->unit - 1) / sp->unit
+                             : 0;
+  static_assert(gpr_ctx::kPinnedChunk / gpr_ctx::kScanUnit <= (size_t)gpr_ctx::kMarkBlocks, "a chunk's units fit the ring");
   // pinned and device sources need no staging copy: one producer keeps the DMA engine busy
   sp->nt = sp->staged ? (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)ctx->up_threads, sp->n_chunks)) : 1;
   if (sp->staged && !ctx->h_up_ring)
@@ -1693,41 +1711,45 @@ int gpr_text_scan_next(gpr_ctx* ctx, uint64_t* opens, uint64_t* closes, uint64_t
   ScanPipe* sp = ctx->pipe;
   if (!sp) return fail(ctx, GPR_E_STATE, "no scan in progress (gpr_text_scan_begin)");
   *n_opens = *n_closes = 0;
-  if (sp->next >= sp->n_chunks) {  // everything delivered (also: empty text)
+  if (sp->next >= sp->n_units) {  // everything delivered (also: empty text)
     *bytes_done = sp->n, *more = 0;
     return scan_pipe_finish(ctx, true);
   }
   constexpr int NB = gpr_ctx::kMarkBlocks;
-  const uint64_t c = sp->next;
-  while (sp->recorded[c % NB].load(std::memory_order_acquire) != c + 1) {
+  const uint64_t u = sp->next;
+  while (sp->recorded[u % NB].load(std::memory_order_acquire) != u + 1) {
     if (sp->error.load() || sp->stop.load()) return scan_pipe_finish(ctx, false) != GPR_OK ? GPR_E_CUDA : fail(ctx, GPR_E_CUDA, "text upload stopped");
     std::this_thread::yield();
   }
   CU(cudaSetDevice(ctx->device));
-  cudaError_t e = cudaEventSynchronize(ctx->mark_event[c % NB]);
+  cudaError_t e = cudaEventSynchronize(ctx->mark_event[u % NB]);
   if (e != cudaSuccess) {
     (void)scan_pipe_finish(ctx, false);
     return fail(ctx, GPR_E_CUDA, "text scan: %s", cudaGetErrorString(e));
   }
-  const uint32_t* block = ctx->h_mark_blocks + (size_t)(c % NB) * kBlockWords;
-  const uint64_t no = block[0], nc = block[1], base = c * sp->chunk;
+  const uint32_t* block = ctx->h_mark_blocks + (size_t)(u % NB) * kBlockWords;
+  const uint64_t c = u / sp->units_per_chunk;
+  const uint64_t base = c * sp->chunk + (u % sp->units_per_chunk) * sp->unit;
+  const uint64_t end = std::min<uint64_t>({sp->n, (c + 1) * sp->chunk, base + sp->unit});
+  const uint64_t no = block[0], nc = block[1];
   if (no > gpr_ctx::kMarkCap || nc > gpr_ctx::kMarkCap || no > cap || nc > cap) {
     const bool caller = no <= gpr_ctx::kMarkCap && nc <= gpr_ctx::kMarkCap;
     *n_opens = no, *n_closes = nc;
     if (!caller) (void)scan_pipe_finish(ctx, false);  // (a too small `cap` may be retried with a larger one)
-    return fail(ctx, GPR_E_CAPACITY, "%llu / %llu markers in one %llu-byte chunk, room for %llu", (unsigned long long)no,
-                (unsigned long long)nc, (unsigned long long)sp->chunk, (unsigned long long)(caller ? cap : gpr_ctx::kMarkCap));
+    return fail(ctx, GPR_E_CAPACITY, "%llu / %llu markers in the %llu bytes of text at offset %llu, room for %llu",
+                (unsigned long long)no, (unsigned long long)nc, (unsigned long long)(end - base), (unsigned long long)base,
+                (unsigned long long)(caller ? cap : gpr_ctx::kMarkCap));
   }
   for (uint64_t i = 0; i < no; ++i) opens[i] = base + block[2 + i];
   for (uint64_t i = 0; i < nc; ++i) closes[i] = base + block[2 + gpr_ctx::kMarkCap + i];
   std::sort(opens, opens + no);
   std::sort(closes, closes + nc);
   *n_opens = no, *n_closes = nc;
-  sp->next = c + 1;
-  sp->consumed.store(c + 1, std::memory_order_release);
-  *bytes_done = std::min<uint64_t>(sp->n, (c + 1) * sp->chunk);
+  sp->next = u + 1;
+  sp->consumed.store(u + 1, std::memory_order_release);
+  *bytes_done = end;
   *more = 1;
-  if (sp->next >= sp->n_chunks) {
+  if (sp->next >= sp->n_units) {
     *more = 0;
     return scan_pipe_finish(ctx, true);
   }

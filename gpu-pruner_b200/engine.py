@@ -396,14 +396,15 @@ class IdleEngine:
             no, nc = C.c_uint64(0), C.c_uint64(0)
             rc = self._lib.gpr_text_scan(self._h, slot, _ptr(buf), n, mem_kind, _ptr(opens), _ptr(closes), cap,
                                          C.byref(no), C.byref(nc))
-            if rc == ffi.GPR_E_CAPACITY:
+            if rc == ffi.GPR_E_CAPACITY and max(no.value, nc.value) > cap:   # our cap was short: ask again
                 cap = int(max(no.value, nc.value)) + 16
                 continue
+            # (otherwise a piece of the text held more markers than the scan has room for: raise)
             self._check(rc)
             return np.sort(opens[:no.value]), np.sort(closes[:nc.value])
 
     def text_scan_chunks(self, text, slot: int = 0, n_bytes: Optional[int] = None, mem_kind: int = ffi.GPR_MEM_HOST):
-        """generator over the pipelined scan: yields (opens, closes, bytes_done) per 4 MB chunk while later chunks are
+        """generator over the pipelined scan: yields (opens, closes, bytes_done) per piece of at most 2 MB while later chunks are
         still being uploaded (gpr_text_scan_begin / gpr_text_scan_next)"""
         buf = np.frombuffer(text, dtype=np.uint8) if isinstance(text, (bytes, bytearray)) else text
         n = int(buf.size if n_bytes is None else n_bytes)

@@ -410,16 +410,23 @@ typedef struct gpr_text_grid {
  * full PCIe speed; ordinary memory is staged through a pinned ring by a few host threads, and every
  * chunk is scanned as it lands) and scan it.  Up to `cap` offsets are written to each of opens[]
  * (position of the '}' of `},"values":[`) and closes[] (position of the '"' of `"]]`), UNSORTED; the
- * true counts are returned in *n_opens / *n_closes (GPR_E_CAPACITY if either exceeds cap).  The text
- * stays resident in the context's slot `slot` (0..2: a tick has up to three responses — PROF, UTIL,
- * POWER) for gpr_text_parse until the next gpr_text_scan of that slot.  Blocking.                   */
+ * true counts are returned in *n_opens / *n_closes (GPR_E_CAPACITY if either exceeds cap; call again
+ * with a larger one).  The scan itself has room for 16,384 markers of each kind in every piece of the
+ * text (gpr_text_scan_next): one per 128 bytes, for every source memory and GPR_TEXT_CHUNK_MB.  A text
+ * whose `},"values":[` and whose `"]]` are each at least 128 bytes apart always fits; a denser piece
+ * fails the scan with GPR_E_CAPACITY naming the piece (the text is not malformed: parse it on the CPU).
+ * The text stays resident in the context's slot `slot` (0..2: a tick has up to three responses — PROF,
+ * UTIL, POWER) for gpr_text_parse until the next gpr_text_scan of that slot.  Blocking.              */
 GPR_API int gpr_text_scan(gpr_ctx *ctx, int32_t slot, const char *text, uint64_t n_bytes,
                           int32_t mem_kind, uint64_t *opens, uint64_t *closes, uint64_t cap,
                           uint64_t *n_opens, uint64_t *n_closes);
 /* The same, as a pipeline the caller can work alongside: gpr_text_scan_begin starts the upload (producer threads
- * owned by the library) and returns; every gpr_text_scan_next blocks until the next chunk of the text (2 MB; 16 MB
- * for pinned text) has landed and been scanned and returns that chunk's markers (sorted; room for `cap` of each
- * kind — 16,384 always suffices) together with *bytes_done = how much of the text is covered so far.  *more = 0 with the last chunk
+ * owned by the library) and returns; every gpr_text_scan_next blocks until the next piece of the text (2 MB; 1 MB
+ * for pageable text at GPR_TEXT_CHUNK_MB=1) has landed and been scanned and returns that piece's markers (sorted;
+ * room for `cap` of each kind — 16,384 always suffices) together with *bytes_done = how much of the text is covered
+ * so far.  A piece with more than `cap` markers of a kind returns GPR_E_CAPACITY with its true counts and may be
+ * asked for again with a larger cap; a piece with more than 16,384 (markers less than 128 bytes apart on average)
+ * returns GPR_E_CAPACITY and ends the scan.  *more = 0 with the last piece
  * (or at once for an empty text); the scan is then complete and the text ready for gpr_text_parse.  Between the
  * calls the caller can already walk the series whose markers it has (gpu-pruner_b200/host/ingest_device.cpp turns
  * label maps into tensor rows while later chunks are still crossing PCIe).  Dropped by the next
