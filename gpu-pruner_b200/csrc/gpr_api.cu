@@ -31,6 +31,7 @@
 #include "gpr_ring.cuh"
 #include "gpr_synth.cuh"
 #include "gpr_text_kernels.cuh"
+#include "gpr_samples.cuh"
 
 namespace {
 
@@ -216,6 +217,18 @@ struct gpr_ctx {
   cudaEvent_t mark_event[kMarkBlocks] = {};
   int up_threads = 8;                  // GPR_TEXT_UPLOAD_THREADS (1..16)
   struct ScanPipe* pipe = nullptr;     // the scan in progress (gpr_text_scan_begin .. last gpr_text_scan_next)
+
+  // decoded samples (gpr_samples_scatter).  A host batch goes up in pieces of gpr::samples::kHostPiece samples through
+  // two device buffers (and, for pageable memory, two pinned ones): piece k + 1 is copied while piece k is scattered.
+  uint64_t* d_soffsets = nullptr;      // a host batch's offsets and rows, uploaded whole (12 B per series)
+  size_t soffsets_cap = 0;
+  uint32_t* d_srows = nullptr;
+  size_t srows_cap = 0;
+  unsigned long long* d_sstats = nullptr;  // [n_oow, n_tiny, check word of a device batch]
+  unsigned char* d_sstage = nullptr;   // [2][ts kHostPiece | values kHostPiece]
+  unsigned char* h_sstage = nullptr;   // the same, pinned
+  cudaEvent_t ev_sup[2] = {};          // piece in buffer b uploaded
+  cudaEvent_t ev_sdone[2] = {};        // piece in buffer b scattered
 
   // multi-GPU
   ncclComm_t comm = nullptr;
@@ -967,6 +980,61 @@ int scan_pipe_finish(gpr_ctx* ctx, bool ok) {
   return GPR_OK;
 }
 
+// the time axis of a gpr_text_grid, as gpr_text_parse and gpr_samples_scatter check it
+int check_grid(gpr_ctx* ctx, const gpr_text_grid* grid) {
+  if (grid->step <= 0 || grid->step > 4000000ll || grid->n_samples == 0 || grid->window_seconds <= 0 ||
+      grid->window_seconds > 4000000000ll)
+    return fail(ctx, GPR_E_INVALID, "step (<= 4e6 s), window_seconds and n_samples must be > 0");
+  if ((grid->window_seconds + grid->step - 1) / grid->step > (int64_t)grid->n_samples)
+    return fail(ctx, GPR_E_INVALID, "window of %lld s needs more than %u columns of %lld s", (long long)grid->window_seconds,
+                grid->n_samples, (long long)grid->step);
+  return GPR_OK;
+}
+
+// Where gpr_text_parse and gpr_samples_scatter merge samples, and its time axis in milliseconds (the resolution of
+// Prometheus timestamps): the resident ring (GPR_TEXT_RESIDENT) or the context plane `plane`, grown to the grid
+// (a plane that has to grow must be filled).  Writes no cell: filling the plane (GPR_TEXT_FILL) and marking the
+// ring's index stale are the caller's.
+int text_destination(gpr_ctx* ctx, const gpr_text_grid* grid, int32_t plane, gpr::text::Grid* g, float** pl) {
+  const uint32_t n_samples = grid->n_samples, n_rows = grid->n_rows;
+  memset(g, 0, sizeof *g);
+  g->t_end = grid->t_end * 1000, g->t_lo = (grid->t_end - grid->window_seconds) * 1000;
+  g->step = (uint32_t)(grid->step * 1000), g->T = n_samples;
+  g->power = gpr::text::power_snap(plane == 1 ? grid->power_threshold : 0.0);
+  if (grid->flags & GPR_TEXT_RESIDENT) {
+    if (!ctx->d_res_util) return fail(ctx, GPR_E_STATE, "no resident window (gpr_resident_init)");
+    if (n_samples != ctx->res_T || (uint64_t)n_rows > (uint64_t)ctx->res_P * ctx->res_G)
+      return fail(ctx, GPR_E_INVALID, "grid %u rows x %u does not match the resident window (%u x %u)", n_rows, n_samples,
+                  ctx->res_P * ctx->res_G, ctx->res_T);
+    *pl = plane == 0 ? ctx->d_res_util : ctx->d_res_power;
+    if (!*pl) return fail(ctx, GPR_E_STATE, "the resident window has no power plane");
+    g->ld = ctx->res_T;
+    g->col_end = (ctx->res_head + ctx->res_T - 1) % ctx->res_T;  // the newest bucket sits just before the head
+  } else {
+    const size_t cells = (size_t)n_rows * n_samples;
+    const size_t cap_before = ctx->tplane_cap[plane];
+    int rc;
+    if ((rc = grow(ctx, &ctx->d_tplane[plane], &ctx->tplane_cap[plane], cells + 4)) != GPR_OK) return rc;
+    if (ctx->tplane_cap[plane] != cap_before && !(grid->flags & GPR_TEXT_FILL))
+      return fail(ctx, GPR_E_STATE, "plane %d had to grow: the first parse of a window must pass GPR_TEXT_FILL", plane);
+    *pl = ctx->d_tplane[plane];
+    g->ld = n_samples, g->col_end = n_samples - 1;
+  }
+  return GPR_OK;
+}
+
+// the fill of a context plane (GPR_TEXT_FILL) and the stale mark of the ring's index, once the merge is certain
+int open_destination(gpr_ctx* ctx, const gpr_text_grid* grid, float* pl) {
+  if (grid->flags & GPR_TEXT_RESIDENT) {
+    if (ctx->d_idx_util) ctx->idx_stale = true;  // the merge does not touch the index (gpr_resident_reindex)
+  } else if (grid->flags & GPR_TEXT_FILL) {
+    // 0xFFFFFFFF: a NaN, and -1 as an int — below every non-negative sample for the integer atomicMax merge
+    const size_t cells = (size_t)grid->n_rows * grid->n_samples;
+    if (cells) CU(cudaMemsetAsync(pl, 0xFF, cells * sizeof(float), ctx->stream));
+  }
+  return GPR_OK;
+}
+
 }  // namespace
 
 void scan_pipe_abort(gpr_ctx* ctx) {
@@ -1010,10 +1078,16 @@ void gpr_destroy(gpr_ctx* ctx) {
                  ctx->d_idx_util,   ctx->d_idx_power,   ctx->d_text[0],    ctx->d_text[1],
                  ctx->d_text[2],    ctx->d_marks,       ctx->d_mark_counts, ctx->d_spans,
                  ctx->d_tplane[0],  ctx->d_tplane[1],  ctx->d_grouped,   ctx->d_gpods,
-                 ctx->d_gmax,       ctx->d_gtable,     ctx->d_islots};
+                 ctx->d_gmax,       ctx->d_gtable,     ctx->d_islots,    ctx->d_soffsets,
+                 ctx->d_srows,      ctx->d_sstats,     ctx->d_sstage};
   for (void* p : dev)
     if (p) cudaFree(p);
   if (ctx->h_counts) cudaFreeHost(ctx->h_counts);
+  if (ctx->h_sstage) cudaFreeHost(ctx->h_sstage);
+  for (int b = 0; b < 2; ++b) {
+    if (ctx->ev_sup[b]) cudaEventDestroy(ctx->ev_sup[b]);
+    if (ctx->ev_sdone[b]) cudaEventDestroy(ctx->ev_sdone[b]);
+  }
   scan_pipe_abort(ctx);
   if (ctx->h_up_ring) cudaFreeHost(ctx->h_up_ring);
   if (ctx->h_mark_blocks) cudaFreeHost(ctx->h_mark_blocks);
@@ -1797,14 +1871,9 @@ int gpr_text_parse(gpr_ctx* ctx, int32_t slot, gpr_text_span* spans, uint32_t n_
   if (slot < 0 || slot > 2 || plane < 0 || plane > 1) return fail(ctx, GPR_E_INVALID, "bad slot %d / plane %d", slot, plane);
   if (!ctx->d_text[slot]) return fail(ctx, GPR_E_STATE, "no text in slot %d (gpr_text_scan)", slot);
   if (n_spans && !spans) return fail(ctx, GPR_E_INVALID, "spans is NULL");
-  const uint32_t n_samples = grid->n_samples, n_rows = grid->n_rows;
-  if (grid->step <= 0 || grid->step > 4000000ll || n_samples == 0 || grid->window_seconds <= 0 ||
-      grid->window_seconds > 4000000000ll)
-    return fail(ctx, GPR_E_INVALID, "step (<= 4e6 s), window_seconds and n_samples must be > 0");
-  if ((grid->window_seconds + grid->step - 1) / grid->step > (int64_t)n_samples)
-    return fail(ctx, GPR_E_INVALID, "window of %lld s needs more than %u columns of %lld s", (long long)grid->window_seconds,
-                n_samples, (long long)grid->step);
-  const bool resident = (grid->flags & GPR_TEXT_RESIDENT) != 0;
+  const uint32_t n_rows = grid->n_rows;
+  int rc;
+  if ((rc = check_grid(ctx, grid)) != GPR_OK) return rc;
   const uint64_t n = ctx->text_n[slot];
   for (uint32_t i = 0; i < n_spans; ++i) {
     if (spans[i].begin > spans[i].end || spans[i].end > n || spans[i].row >= n_rows ||
@@ -1814,35 +1883,10 @@ int gpr_text_parse(gpr_ctx* ctx, int32_t slot, gpr_text_span* spans, uint32_t n_
     spans[i].n_in = spans[i].n_oow = spans[i].n_tiny = 0;
   }
   CU(cudaSetDevice(ctx->device));
-  int rc;
   float* pl = nullptr;
   gpr::text::Grid g;
-  memset(&g, 0, sizeof g);
-  // the device works in milliseconds, the resolution of Prometheus timestamps
-  g.t_end = grid->t_end * 1000, g.t_lo = (grid->t_end - grid->window_seconds) * 1000;
-  g.step = (uint32_t)(grid->step * 1000), g.T = n_samples;
-  g.power = gpr::text::power_snap(plane == 1 ? grid->power_threshold : 0.0);
-  if (resident) {
-    if (!ctx->d_res_util) return fail(ctx, GPR_E_STATE, "no resident window (gpr_resident_init)");
-    if (n_samples != ctx->res_T || (uint64_t)n_rows > (uint64_t)ctx->res_P * ctx->res_G)
-      return fail(ctx, GPR_E_INVALID, "grid %u rows x %u does not match the resident window (%u x %u)", n_rows, n_samples,
-                  ctx->res_P * ctx->res_G, ctx->res_T);
-    pl = plane == 0 ? ctx->d_res_util : ctx->d_res_power;
-    if (!pl) return fail(ctx, GPR_E_STATE, "the resident window has no power plane");
-    g.ld = ctx->res_T;
-    g.col_end = (ctx->res_head + ctx->res_T - 1) % ctx->res_T;  // the newest bucket sits just before the head
-    if (ctx->d_idx_util) ctx->idx_stale = true;  // the merge does not touch the index (gpr_resident_reindex)
-  } else {
-    const size_t cells = (size_t)n_rows * n_samples;
-    const size_t cap_before = ctx->tplane_cap[plane];
-    if ((rc = grow(ctx, &ctx->d_tplane[plane], &ctx->tplane_cap[plane], cells + 4)) != GPR_OK) return rc;
-    if (ctx->tplane_cap[plane] != cap_before && !(grid->flags & GPR_TEXT_FILL))
-      return fail(ctx, GPR_E_STATE, "plane %d had to grow: the first parse of a window must pass GPR_TEXT_FILL", plane);
-    pl = ctx->d_tplane[plane];
-    g.ld = n_samples, g.col_end = n_samples - 1;
-    // 0xFFFFFFFF: a NaN, and -1 as an int — below every non-negative sample for the integer atomicMax merge
-    if ((grid->flags & GPR_TEXT_FILL) && cells) CU(cudaMemsetAsync(pl, 0xFF, cells * sizeof(float), ctx->stream));
-  }
+  if ((rc = text_destination(ctx, grid, plane, &g, &pl)) != GPR_OK) return rc;
+  if ((rc = open_destination(ctx, grid, pl)) != GPR_OK) return rc;
   if ((rc = grow(ctx, &ctx->d_spans, &ctx->spans_cap, (size_t)n_spans + 1)) != GPR_OK) return rc;
   ctx->last_was_reduce = false;
   if (n_spans && n) {
@@ -1868,6 +1912,143 @@ int gpr_text_planes(gpr_ctx* ctx, float** util, float** power) {
   if (util) *util = ctx->d_tplane[0];
   if (power) *power = ctx->d_tplane[1];
   return GPR_OK;
+}
+
+// ---- decoded samples (gpr_samples.cuh) ---------------------------------------------------------------
+static_assert(sizeof(gpr_sample_stats) == 24, "gpr_sample_stats");
+
+static int launch_scatter(gpr_ctx* ctx, const gpr::samples::ScatterArgs& a, bool vec) {
+  namespace gs = gpr::samples;
+  const uint64_t chunks = (a.end - a.base + gs::kChunk - 1) / gs::kChunk;
+  const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(chunks, (uint64_t)ctx->sm_count * 8));
+  if (vec) gs::k_samples_scatter<true><<<grid, gs::kThreads, 0, ctx->stream>>>(a);
+  else gs::k_samples_scatter<false><<<grid, gs::kThreads, 0, ctx->stream>>>(a);
+  ctx->launches++;
+  CU(cudaGetLastError());
+  return GPR_OK;
+}
+
+// A host batch, piece by piece: piece k is copied (through pinned staging if the batch is pageable) into device buffer
+// k % 2 on the copy stream and scattered on the context's stream, so piece k + 1 crosses PCIe while piece k merges.
+static int scatter_host_pieces(gpr_ctx* ctx, const gpr_sample_batch* batch, uint64_t total, gpr::samples::ScatterArgs a) {
+  namespace gs = gpr::samples;
+  const uint32_t S = batch->n_series;
+  int rc;
+  if ((rc = grow(ctx, &ctx->d_soffsets, &ctx->soffsets_cap, (size_t)S + 1)) != GPR_OK) return rc;
+  if ((rc = grow(ctx, &ctx->d_srows, &ctx->srows_cap, (size_t)S + 1)) != GPR_OK) return rc;
+  CU(cudaMemcpyAsync(ctx->d_soffsets, batch->offsets, ((size_t)S + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(ctx->d_srows, batch->rows, (size_t)S * 4, cudaMemcpyHostToDevice, ctx->stream));
+  a.offsets = ctx->d_soffsets, a.rows = ctx->d_srows;
+  bool pinned = true;
+  for (const void* p : {(const void*)batch->ts_ms, (const void*)batch->values}) {
+    cudaPointerAttributes at;
+    pinned = pinned && cudaPointerGetAttributes(&at, p) == cudaSuccess && at.type == cudaMemoryTypeHost;
+    (void)cudaGetLastError();  // an unregistered pointer may leave an error code behind
+  }
+  const size_t half = gs::kHostPiece * 8;  // bytes of one piece's timestamps, or of its values
+  if (!ctx->d_sstage) CU(cudaMalloc(reinterpret_cast<void**>(&ctx->d_sstage), 4 * half));
+  if (!pinned && !ctx->h_sstage) CU(cudaMallocHost(reinterpret_cast<void**>(&ctx->h_sstage), 4 * half));
+  for (int b = 0; b < 2; ++b) {
+    if (!ctx->ev_sup[b]) CU(cudaEventCreateWithFlags(&ctx->ev_sup[b], cudaEventDisableTiming));
+    if (!ctx->ev_sdone[b]) CU(cudaEventCreateWithFlags(&ctx->ev_sdone[b], cudaEventDisableTiming));
+  }
+  uint64_t k = 0;
+  return gs::for_each_piece(batch->offsets, S, total, gs::kHostPiece, [&](const gs::Piece& p) -> int {
+    const int b = (int)(k & 1);
+    const uint64_t n = p.end - p.begin;
+    unsigned char* dst = ctx->d_sstage + (size_t)b * 2 * half;
+    const void* src_t = batch->ts_ms + p.begin;
+    const void* src_v = batch->values + p.begin;
+    if (k >= 2) CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_sdone[b], 0));  // piece k - 2 has left buffer b
+    if (!pinned) {
+      unsigned char* stage = ctx->h_sstage + (size_t)b * 2 * half;
+      if (k >= 2) CU(cudaEventSynchronize(ctx->ev_sup[b]));  // piece k - 2's upload has drained pinned buffer b
+      memcpy(stage, src_t, n * 8);
+      memcpy(stage + half, src_v, n * 8);
+      src_t = stage, src_v = stage + half;
+    }
+    CU(cudaMemcpyAsync(dst, src_t, n * 8, cudaMemcpyHostToDevice, ctx->copy_stream));
+    CU(cudaMemcpyAsync(dst + half, src_v, n * 8, cudaMemcpyHostToDevice, ctx->copy_stream));
+    CU(cudaEventRecord(ctx->ev_sup[b], ctx->copy_stream));
+    CU(cudaStreamWaitEvent(ctx->stream, ctx->ev_sup[b], 0));
+    a.ts = reinterpret_cast<const int64_t*>(dst);
+    a.values = reinterpret_cast<const double*>(dst + half);
+    a.base = p.begin, a.end = p.end, a.s_base = p.series;
+    const int r = launch_scatter(ctx, a, true);
+    if (r != GPR_OK) return r;
+    CU(cudaEventRecord(ctx->ev_sdone[b], ctx->stream));
+    ++k;
+    return GPR_OK;
+  });
+}
+
+int gpr_samples_scatter(gpr_ctx* ctx, const gpr_sample_batch* batch, const gpr_text_grid* grid, int32_t plane,
+                        gpr_sample_stats* stats) {
+  if (!ctx) return GPR_E_INVALID;
+  GPR_TRY
+  NvtxRange nvtx_range("gpr_samples_scatter");
+  namespace gs = gpr::samples;
+  if (!batch || batch->struct_size != sizeof(gpr_sample_batch))
+    return fail(ctx, GPR_E_INVALID, "batch is NULL / struct_size mismatch");
+  if (!grid || grid->struct_size != sizeof(gpr_text_grid)) return fail(ctx, GPR_E_INVALID, "grid is NULL / struct_size mismatch");
+  if (plane < 0 || plane > 1) return fail(ctx, GPR_E_INVALID, "bad plane %d", plane);
+  if (batch->mem_kind != GPR_MEM_HOST && batch->mem_kind != GPR_MEM_DEVICE)
+    return fail(ctx, GPR_E_INVALID, "bad mem_kind %d", batch->mem_kind);
+  int rc;
+  if ((rc = check_grid(ctx, grid)) != GPR_OK) return rc;
+  const uint32_t S = batch->n_series;
+  if (!batch->offsets || (S && !batch->rows)) return fail(ctx, GPR_E_INVALID, "offsets / rows is NULL");
+  CU(cudaSetDevice(ctx->device));
+  ctx->last_was_reduce = false;
+  if (!ctx->d_sstats) CU(cudaMalloc(reinterpret_cast<void**>(&ctx->d_sstats), 4 * sizeof(unsigned long long)));
+  // ---- the batch is checked before anything is written
+  uint32_t bad = 0;
+  uint64_t total = 0;
+  if (batch->mem_kind == GPR_MEM_HOST) {
+    for (uint32_t s = 0; s < std::max(S, 1u); ++s) bad |= gs::series_faults(batch->offsets, batch->rows, S, s, grid->n_rows);
+    total = batch->offsets[S];
+  } else {
+    unsigned long long back[2] = {0, 0};  // the check word, offsets[n_series]
+    CU(cudaMemsetAsync(ctx->d_sstats + 2, 0, sizeof(unsigned long long), ctx->stream));
+    const uint32_t blocks = std::max(1u, std::min((std::max(S, 1u) + 255u) / 256u, (uint32_t)ctx->sm_count * 8u));
+    gs::k_samples_check<<<blocks, 256, 0, ctx->stream>>>(batch->offsets, batch->rows, S, grid->n_rows,
+                                                         reinterpret_cast<unsigned int*>(ctx->d_sstats + 2));
+    ctx->launches++;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(&back[0], ctx->d_sstats + 2, sizeof back[0], cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(&back[1], batch->offsets + S, sizeof back[1], cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    bad = (uint32_t)back[0], total = back[1];
+  }
+  if (bad & gs::kBadStart) return fail(ctx, GPR_E_INVALID, "gpr_sample_batch: offsets[0] != 0");
+  if (bad & gs::kBadOrder) return fail(ctx, GPR_E_INVALID, "gpr_sample_batch: offsets decrease");
+  if (bad & gs::kBadRow) return fail(ctx, GPR_E_INVALID, "gpr_sample_batch: a row >= grid.n_rows (%u)", grid->n_rows);
+  if (total && (!batch->ts_ms || !batch->values)) return fail(ctx, GPR_E_INVALID, "ts_ms / values is NULL");
+  // ---- the destination, then the merge
+  float* pl = nullptr;
+  gs::ScatterArgs a;
+  memset(&a, 0, sizeof a);
+  if ((rc = text_destination(ctx, grid, plane, &a.g, &pl)) != GPR_OK) return rc;
+  if ((rc = open_destination(ctx, grid, pl)) != GPR_OK) return rc;
+  CU(cudaMemsetAsync(ctx->d_sstats, 0, 2 * sizeof(unsigned long long), ctx->stream));
+  a.n_series = S, a.plane = pl, a.stats = ctx->d_sstats;
+  if (total && batch->mem_kind == GPR_MEM_DEVICE) {  // read in place
+    a.offsets = batch->offsets, a.rows = batch->rows, a.ts = batch->ts_ms, a.values = batch->values;
+    a.base = 0, a.end = total, a.s_base = 0;
+    rc = launch_scatter(ctx, a, aligned16(batch->ts_ms) && aligned16(batch->values));
+  } else if (total) {
+    rc = scatter_host_pieces(ctx, batch, total, a);
+  }
+  if (rc != GPR_OK) {
+    (void)cudaStreamSynchronize(ctx->stream);  // the staging buffers may still be read
+    return rc;
+  }
+  unsigned long long counts[2] = {0, 0};
+  CU(cudaMemcpyAsync(counts, ctx->d_sstats, sizeof counts, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  if (stats) stats->n_in = total, stats->n_oow = counts[0], stats->n_tiny = counts[1];
+  return GPR_OK;
+  GPR_CATCH(ctx)
 }
 
 int gpr_synth_fill(gpr_ctx* ctx, uint64_t seed, int32_t plane, float* dst, uint64_t pod_offset,

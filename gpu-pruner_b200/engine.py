@@ -435,6 +435,41 @@ class IdleEngine:
         self._check(self._lib.gpr_text_parse(self._h, slot, _ptr(spans), len(spans), C.byref(g), plane))
         return spans
 
+    def samples_scatter(self, offsets, rows, ts_ms, values, t_end: int, step: int, T: int, n_rows: int, *,
+                        window_seconds: Optional[int] = None, plane: int = 0, resident: bool = False,
+                        fill: bool = True, power_threshold: Optional[float] = 0.0, mem_kind: int = ffi.GPR_MEM_HOST,
+                        n_series: Optional[int] = None) -> dict:
+        """Merge decoded samples into the context's plane (or, ``resident=True``, the resident ring), exactly as
+        :meth:`text_parse` merges the same samples written as text.  CSR form: series s owns samples
+        ``offsets[s]:offsets[s+1]`` (uint64) of ``ts_ms`` (int64 Unix milliseconds) and ``values`` (float64) and
+        feeds row ``rows[s]`` (uint32).  Host arrays (numpy; pinned ones from :meth:`host_array` upload fastest) are
+        converted to those dtypes; with ``mem_kind=GPR_MEM_DEVICE`` pass device addresses / tensors and
+        ``n_series``.  Returns the counts ``{"n_in", "n_oow", "n_tiny"}``."""
+        if mem_kind == ffi.GPR_MEM_HOST:
+            offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+            rows = np.ascontiguousarray(rows, dtype=np.uint32)
+            ts_ms = np.ascontiguousarray(ts_ms, dtype=np.int64)
+            values = np.ascontiguousarray(values, dtype=np.float64)
+            if n_series is None:
+                n_series = rows.size
+        elif n_series is None:
+            raise ValueError("n_series is required for device arrays")
+        b = ffi.gpr_sample_batch()
+        b.struct_size = C.sizeof(ffi.gpr_sample_batch)
+        b.mem_kind = mem_kind
+        b.offsets, b.rows, b.ts_ms, b.values = _ptr(offsets), _ptr(rows), _ptr(ts_ms), _ptr(values)
+        b.n_series = int(n_series)
+        g = ffi.gpr_text_grid()
+        g.struct_size = C.sizeof(ffi.gpr_text_grid)
+        g.flags = (ffi.GPR_TEXT_FILL if fill and not resident else 0) | (ffi.GPR_TEXT_RESIDENT if resident else 0)
+        g.t_end, g.step = int(t_end), int(step)
+        g.window_seconds = int(T) * int(step) if window_seconds is None else int(window_seconds)
+        g.n_samples, g.n_rows = int(T), int(n_rows)
+        g.power_threshold = 0.0 if power_threshold is None else float(power_threshold)
+        st = ffi.gpr_sample_stats()
+        self._check(self._lib.gpr_samples_scatter(self._h, C.byref(b), C.byref(g), plane, C.byref(st)))
+        return {"n_in": st.n_in, "n_oow": st.n_oow, "n_tiny": st.n_tiny}
+
     def resident_head(self) -> int:
         h = C.c_uint32()
         self._check(self._lib.gpr_resident_head(self._h, C.byref(h)))

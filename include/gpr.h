@@ -439,8 +439,59 @@ GPR_API int gpr_text_scan_next(gpr_ctx *ctx, uint64_t *opens, uint64_t *closes, 
 GPR_API int gpr_text_parse(gpr_ctx *ctx, int32_t slot, gpr_text_span *spans, uint32_t n_spans,
                            const gpr_text_grid *grid, int32_t plane);
 /* Device pointers of the context planes (NULL if never parsed); valid until the next gpr_text_parse
- * that has to grow them, or gpr_destroy.  Hand them to gpr_decide with mem_kind = GPR_MEM_DEVICE.   */
+ * or gpr_samples_scatter that has to grow them, or gpr_destroy.  Hand them to gpr_decide with
+ * mem_kind = GPR_MEM_DEVICE.                                                                         */
 GPR_API int gpr_text_planes(gpr_ctx *ctx, float **util, float **power);
+
+/* ---- decoded samples into the same planes -----------------------------------------------------------
+ * For a caller whose Prometheus client has already decoded the range query (prometheus-http-query's
+ * RangeVector: a label map and samples() = [(timestamp f64 s, value f64)] per series): the samples go
+ * straight into a context plane or the resident ring, with every rule of the text path applied on the GPU.
+ *
+ * Samples in CSR form: series s owns samples [offsets[s], offsets[s+1]) and they go to row rows[s] of the
+ * destination (several series may feed one row; samples may come in any order).  Timestamps are Unix
+ * MILLISECONDS.  A Rust caller converts Sample::timestamp() with (ts * 1000.0).round() as i64, which is
+ * exact: Prometheus timestamps are whole milliseconds.  Values are passed as decoded (f64).           */
+struct gpr_sample_batch {
+  uint32_t struct_size;     /* sizeof(gpr_sample_batch)                                                */
+  int32_t mem_kind;         /* GPR_MEM_*: applies to every array below                                 */
+  const uint64_t *offsets;  /* n_series + 1, non-decreasing, offsets[0] = 0                            */
+  const uint32_t *rows;     /* n_series, each < grid.n_rows                                            */
+  const int64_t *ts_ms;     /* offsets[n_series] timestamps, Unix milliseconds (any order)             */
+  const double *values;     /* offsets[n_series] values as decoded (f64)                               */
+  uint32_t n_series;
+  uint32_t reserved;
+};
+typedef struct gpr_sample_batch gpr_sample_batch;
+
+/* n_in: samples in the batch; n_oow: of those, outside the window; n_tiny: in-window non-zero values
+ * below the f32 denormal range, kept non-zero — the sums of gpr_text_span's counters for the same
+ * samples written as text.                                                                          */
+struct gpr_sample_stats {
+  uint64_t n_in;
+  uint64_t n_oow;
+  uint64_t n_tiny;
+};
+typedef struct gpr_sample_stats gpr_sample_stats;
+
+/* Same destination, grid and flags as gpr_text_parse (GPR_TEXT_FILL: a context plane; GPR_TEXT_RESIDENT:
+ * the ring, after gpr_resident_advance; like a text parse it leaves the block index stale, so call
+ * gpr_resident_reindex before gpr_decide_resident).  The cell a sample lands in, and the value it leaves
+ * there, are those gpr_text_parse produces for the same sample written as text ([ts_ms / 1000 as a
+ * decimal, "<value printed round-trip>"]):
+ *   value  to_f32 (rounded to nearest, a non-zero value stays non-zero), and on plane 1 the POWER RULE of
+ *          gpr_window against grid.power_threshold; NaN samples are dropped;
+ *   cell   t_end - window_seconds < ts <= t_end (in ms), bucket (t_end - ts) / step counted back from the
+ *          newest column;
+ *   merge  NaN-aware max, as in the text path.
+ * The batch is checked before anything is written — host arrays on the host, device arrays by a kernel
+ * whose verdict is read back first: a bad struct_size, offsets[0] != 0, decreasing offsets or a row
+ * >= grid.n_rows returns GPR_E_INVALID and leaves the destination untouched.  GPR_TEXT_RESIDENT without a
+ * resident window is GPR_E_STATE.  Device arrays are read in place; host arrays (pinned from
+ * gpr_host_alloc, or pageable) are uploaded in pieces that overlap with the scatter, so a batch needs no
+ * device copy of itself.  stats may be NULL.  Blocking; results enqueued before the call stay pending.   */
+GPR_API int gpr_samples_scatter(gpr_ctx *ctx, const gpr_sample_batch *batch, const gpr_text_grid *grid,
+                                int32_t plane, gpr_sample_stats *stats);
 
 #ifdef __cplusplus
 }
