@@ -93,16 +93,73 @@ struct Pending {
   int slot;
 };
 
+// ---- what a context owns: every buffer, event and stream of a gpr_ctx is one of these and releases itself when the
+// context is deleted, so gpr_destroy lists none of them.  A buffer counts in elements of T and lives in device memory,
+// or (kPinned) in pinned host memory from cudaHostAlloc with the given flags.
+template <typename T, bool kPinned = false>
+struct Buf {
+  T* p = nullptr;
+  size_t cap = 0;
+  Buf() = default;
+  Buf(const Buf&) = delete;
+  Buf& operator=(const Buf&) = delete;
+  ~Buf() { release(); }
+  operator T*() const { return p; }
+  cudaError_t release() {
+    const cudaError_t e = !p ? cudaSuccess : kPinned ? cudaFreeHost(p) : cudaFree(p);
+    p = nullptr, cap = 0;
+    return e;
+  }
+  // exactly n elements in place of what is held (nothing may still use it)
+  cudaError_t alloc(size_t n, unsigned flags = cudaHostAllocDefault) {
+    cudaError_t e = release();
+    void* q = nullptr;
+    if (e == cudaSuccess) e = kPinned ? cudaHostAlloc(&q, n * sizeof(T), flags) : cudaMalloc(&q, n * sizeof(T));
+    if (e == cudaSuccess) p = static_cast<T*>(q), cap = n;
+    return e;
+  }
+  // n elements on first use; later calls keep what is held
+  cudaError_t alloc_once(size_t n, unsigned flags = cudaHostAllocDefault) { return p ? cudaSuccess : alloc(n, flags); }
+  // The growth rule of the context's scratch: nothing happens while cap >= need.  Otherwise the work on `st` that may
+  // still read the buffer is waited for and need + need / 4 + 64 elements replace it (a caller that must know
+  // whether it grew compares cap).
+  cudaError_t grow(cudaStream_t st, size_t need) {
+    if (need <= cap) return cudaSuccess;
+    if (p) {
+      const cudaError_t e = cudaStreamSynchronize(st);
+      if (e != cudaSuccess) return e;
+    }
+    return alloc(need + need / 4 + 64);
+  }
+};
+template <typename T>
+using PinnedBuf = Buf<T, true>;
+
+// an event or a stream; create() makes it on first use and keeps it after
+template <typename H, cudaError_t (*Create)(H*, unsigned), cudaError_t (*Destroy)(H)>
+struct Handle {
+  H h = nullptr;
+  Handle() = default;
+  Handle(const Handle&) = delete;
+  Handle& operator=(const Handle&) = delete;
+  ~Handle() {
+    if (h) Destroy(h);
+  }
+  operator H() const { return h; }
+  cudaError_t create(unsigned flags) { return h ? cudaSuccess : Create(&h, flags); }
+};
+using Event = Handle<cudaEvent_t, cudaEventCreateWithFlags, cudaEventDestroy>;
+using Stream = Handle<cudaStream_t, cudaStreamCreateWithFlags, cudaStreamDestroy>;
+
 }  // namespace
 
 struct gpr_ctx {
   int device = 0;
-  cudaStream_t stream = nullptr;
+  cudaStream_t stream = nullptr;  // the caller's (never destroyed here) unless own_stream
   bool own_stream = false;
-  cudaStream_t copy_stream = nullptr;
-  cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr, ev_t0 = nullptr, ev_t1 = nullptr;
-  cudaEvent_t ev_join = nullptr;
-  cudaEvent_t ev_chunk[kMaxChunkEvents] = {};
+  Stream copy_stream;
+  Event ev_k0, ev_k1, ev_t0, ev_t1, ev_join;
+  Event ev_chunk[kMaxChunkEvents];
   int sm_count = 0;
   size_t l2_bytes = 0, hbm_bytes = 0;
   int cc_major = 0, cc_minor = 0;
@@ -118,44 +175,34 @@ struct gpr_ctx {
   // capacity for host windows
   uint32_t max_pods = 0, max_gpus = 0, max_samples = 0;
   bool cap_power = false;
-  float* d_util_stage = nullptr;
-  float* d_power_stage = nullptr;
-  uint8_t* d_elig_stage = nullptr;
-  int64_t* d_created_stage = nullptr;
-  size_t gate_cap = 0;
+  Buf<float> d_util_stage;
+  Buf<float> d_power_stage;
+  Buf<uint8_t> d_elig_stage;
+  Buf<int64_t> d_created_stage;
 
   // scratch (grown on demand)
   // Two scratch sets used alternately by successive single-launch decisions so that a launch may
   // start (programmatic dependent launch) while its predecessor is still folding.
-  uint32_t* d_masks[2] = {nullptr, nullptr};  // each [idle P | veto P], all-zero between uses
-  size_t masks_cap[2] = {0, 0};
+  Buf<uint32_t> d_masks[2];     // each [idle P | veto P], all-zero between uses
   bool masks_dirty = false;     // a failed call may have left bits behind
-  unsigned int* d_tickets = nullptr;          // [2] fold-grid tickets
-  unsigned long long* d_acc = nullptr;        // [2][3] fold-grid count accumulators
-  unsigned long long* d_done = nullptr;       // [2] completed folds per scratch set
+  Buf<unsigned int> d_tickets;          // [2] fold-grid tickets
+  Buf<unsigned long long> d_acc;        // [2][3] fold-grid count accumulators
+  Buf<unsigned long long> d_done;       // [2] completed folds per scratch set
   unsigned long long uses[2] = {0, 0};        // folds issued per scratch set
   unsigned parity = 0;
   bool pdl_enabled = true;      // GPR_PDL=0 disables programmatic dependent launch
   bool last_was_reduce = false; // the newest op on the stream is one of our fold kernels
-  uint32_t* d_bits = nullptr;  // [dbits W | cbits W]
-  size_t bits_cap = 0;
-  uint32_t* d_gather = nullptr;  // [world][2W]
-  size_t gather_cap = 0;
-  float* d_smax = nullptr;
-  size_t smax_cap = 0;
+  Buf<uint32_t> d_bits;    // [dbits W | cbits W]
+  Buf<uint32_t> d_gather;  // [world][2W]
+  Buf<float> d_smax;
   // `sum by` groups (gpr_window.groups, gpr_groups.cuh): single-buffered, so a decision with a table runs without PDL
-  uint32_t* d_grouped = nullptr;   // [P][MW] rows of groups of two or more
-  size_t grouped_cap = 0;
-  uint32_t* d_gpods = nullptr;     // [1 + P]: count, then the pods with such groups
-  size_t gpods_cap = 0;
-  float* d_gmax = nullptr;         // [P*G] max of the grouped rows when the caller did not ask for series_max
-  size_t gmax_cap = 0;
-  uint32_t* d_gtable = nullptr;    // [P*G] a host table, uploaded
-  size_t gtable_cap = 0;
-  uint32_t* d_islots = nullptr;    // [P][MW] idle_slots for host outputs
-  size_t islots_cap = 0;
+  Buf<uint32_t> d_grouped;   // [P][MW] rows of groups of two or more
+  Buf<uint32_t> d_gpods;     // [1 + P]: count, then the pods with such groups
+  Buf<float> d_gmax;         // [P*G] max of the grouped rows when the caller did not ask for series_max
+  Buf<uint32_t> d_gtable;    // [P*G] a host table, uploaded
+  Buf<uint32_t> d_islots;    // [P][MW] idle_slots for host outputs
   unsigned int* h_gerr = nullptr;  // host-mapped: 1 + a pod whose device group table is malformed
-  unsigned long long* h_counts = nullptr;  // pinned [kSlots][4]: n_series, n_candidates, n_decisions,
+  PinnedBuf<unsigned long long> h_counts;  // [kSlots][4]: n_series, n_candidates, n_decisions,
                                            // %globaltimer at completion; then [mark, error word]
   unsigned long long* h_mark = nullptr;    // %globaltimer written by the last gpr_timer_begin
   unsigned int* h_err = nullptr;           // raised by a kernel whose peer wait timed out (h_gerr is the next word)
@@ -164,36 +211,28 @@ struct gpr_ctx {
   std::vector<uint64_t> phase_stamps;      // 4 per decision: fold start, folded, flags raised, peers arrived
   unsigned long long rdv_seq = 0;          // rendezvous sequence number (same on all ranks)
 
-  void* d_flush = nullptr;
-  size_t flush_bytes = 0;
+  Buf<unsigned char> d_flush;
 
   // resident window (daemon mode)
-  float* d_res_util = nullptr;
-  float* d_res_power = nullptr;
+  Buf<float> d_res_util;
+  Buf<float> d_res_power;
   uint32_t res_P = 0, res_G = 0, res_T = 0, res_head = 0;
   // optional index (GPR_F_BLOCK_INDEX): max of every 64-sample block of every resident row, kept up to
   // date by gpr_append.  max-of-block-maxima == max-of-samples (NaN = block without a sample), so the
   // index is itself a window tensor with ceil(T/64) "samples" per series and the same kernels decide on it
-  float* d_idx_util = nullptr;
-  float* d_idx_power = nullptr;
+  Buf<float> d_idx_util;
+  Buf<float> d_idx_power;
   uint32_t idx_ld = 0;      // padded to a multiple of 4 (TMA-able rows), padding stays NaN
   // gpr_text_parse(GPR_TEXT_RESIDENT) merged samples into the ring behind the index's back: deciding on the index
   // is refused until gpr_resident_reindex has rebuilt it
   bool idx_stale = false;
-  float* d_cols = nullptr;
-  size_t cols_cap = 0;
+  Buf<float> d_cols;
 
   // device-side ingest of response text (gpr_text_scan / gpr_text_parse)
-  uint8_t* d_text[3] = {nullptr, nullptr, nullptr};
-  size_t text_cap[3] = {0, 0, 0};
+  Buf<uint8_t> d_text[3];
   uint64_t text_n[3] = {0, 0, 0};
-  uint64_t* d_marks = nullptr;  // [2][marks_cap]
-  size_t marks_cap = 0;         // total entries (both lists)
-  unsigned long long* d_mark_counts = nullptr;
-  gpr::text::Span* d_spans = nullptr;
-  size_t spans_cap = 0;
-  float* d_tplane[2] = {nullptr, nullptr};
-  size_t tplane_cap[2] = {0, 0};
+  Buf<gpr::text::Span> d_spans;
+  Buf<float> d_tplane[2];
   // The text goes up in chunks through a few producer threads (pageable text is staged through a small pinned
   // ring) and every chunk is scanned as soon as it has landed; the markers of a chunk are written by the scan
   // kernel straight into a block of mapped pinned memory (ScanPipe, gpr_text_scan_begin / _next).
@@ -209,32 +248,30 @@ struct gpr_ctx {
   static constexpr uint32_t kMarkCap = 16384;              // markers of one kind per unit (2 MB: one per 128 B)
   size_t up_chunk = 2u << 20;
   size_t up_slot_bytes = 0;            // up_chunk + a page (the 16 bytes of overlap, page aligned)
-  unsigned char* h_up_ring = nullptr;  // [up_threads][kUpSlots][up_slot_bytes], pinned
-  uint32_t* h_mark_blocks = nullptr;   // [kMarkBlocks][2 + 2 * kMarkCap], pinned + device-mapped (8 MB)
-  uint32_t* d_mark_blocks = nullptr;   // the same in device memory: the scan appends here (atomics), then publishes
-  cudaStream_t up_stream[kUpThreads] = {};
-  cudaEvent_t up_event[kUpThreads][kUpSlots] = {};
-  cudaEvent_t mark_event[kMarkBlocks] = {};
+  PinnedBuf<unsigned char> h_up_ring;  // [up_threads][kUpSlots][up_slot_bytes]
+  PinnedBuf<uint32_t> h_mark_blocks;   // [kMarkBlocks][2 + 2 * kMarkCap], device-mapped (8 MB)
+  Buf<uint32_t> d_mark_blocks;         // the same in device memory: the scan appends here (atomics), then publishes
+  Stream up_stream[kUpThreads];
+  Event up_event[kUpThreads][kUpSlots];
+  Event mark_event[kMarkBlocks];
   int up_threads = 8;                  // GPR_TEXT_UPLOAD_THREADS (1..16)
   struct ScanPipe* pipe = nullptr;     // the scan in progress (gpr_text_scan_begin .. last gpr_text_scan_next)
 
   // decoded samples (gpr_samples_scatter).  A host batch goes up in pieces of gpr::samples::kHostPiece samples through
   // two device buffers (and, for pageable memory, two pinned ones): piece k + 1 is copied while piece k is scattered.
-  uint64_t* d_soffsets = nullptr;      // a host batch's offsets and rows, uploaded whole (12 B per series)
-  size_t soffsets_cap = 0;
-  uint32_t* d_srows = nullptr;
-  size_t srows_cap = 0;
-  unsigned long long* d_sstats = nullptr;  // [n_oow, n_tiny, check word of a device batch]
-  unsigned char* d_sstage = nullptr;   // [2][ts kHostPiece | values kHostPiece]
-  unsigned char* h_sstage = nullptr;   // the same, pinned
-  cudaEvent_t ev_sup[2] = {};          // piece in buffer b uploaded
-  cudaEvent_t ev_sdone[2] = {};        // piece in buffer b scattered
+  Buf<uint64_t> d_soffsets;            // a host batch's offsets and rows, uploaded whole (12 B per series)
+  Buf<uint32_t> d_srows;
+  Buf<unsigned long long> d_sstats;    // [n_oow, n_tiny, check word of a device batch]
+  Buf<unsigned char> d_sstage;         // [2][ts kHostPiece | values kHostPiece]
+  PinnedBuf<unsigned char> h_sstage;   // the same, pinned
+  Event ev_sup[2];                     // piece in buffer b uploaded
+  Event ev_sdone[2];                   // piece in buffer b scattered
 
   // multi-GPU
   ncclComm_t comm = nullptr;
   int rank = 0, world = 1;
   // fused exchange over peer memory (gpr_p2p_init / gpr_p2p_attach)
-  unsigned char* p2p_block = nullptr;            // [flags u64 x kMaxPeers | rendezvous flags | gather[4][world][stride] | slots[4][world][stride]]
+  Buf<unsigned char> p2p_block;                  // [flags u64 x kMaxPeers | rendezvous flags | gather[4][world][stride] | slots[4][world][stride]]
   unsigned char* p2p_peer[gpr::kMaxPeers] = {};  // peer-mapped base of every rank's block (self = local)
   // Exchange buffers are kExchangeDepth deep (step % depth), twice the number of scratch sets: with the late
   // output ordering a rank may push step n + 4 only after every peer has consumed step n (see k_fold)
@@ -287,21 +324,6 @@ int fail(gpr_ctx* c, int code, const char* fmt, ...) {
     if (r_ != ncclSuccess)                                                                \
       return fail(ctx, GPR_E_NCCL, "%s: %s", #call, g_nccl.GetErrorString(r_));           \
   } while (0)
-
-template <typename T>
-int grow(gpr_ctx* ctx, T** p, size_t* cap, size_t need) {
-  if (need <= *cap) return GPR_OK;
-  if (*p) {
-    CU(cudaStreamSynchronize(ctx->stream));
-    CU(cudaFree(*p));
-    *p = nullptr;
-    *cap = 0;
-  }
-  size_t want = need + need / 4 + 64;
-  CU(cudaMalloc(reinterpret_cast<void**>(p), want * sizeof(T)));
-  *cap = want;
-  return GPR_OK;
-}
 
 int env_int(const char* name, int dflt) {
   const char* v = getenv(name);
@@ -497,49 +519,33 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
     ctx->last_was_reduce = false;
   }
   for (int k = 0; k < 2; ++k) {
-    const size_t cap_before = ctx->masks_cap[k];
-    if ((rc = grow(ctx, &ctx->d_masks[k], &ctx->masks_cap[k], (size_t)2 * P * MW + 16)) != GPR_OK) return rc;
-    if (ctx->masks_cap[k] != cap_before || ctx->masks_dirty) {
-      CU(cudaMemsetAsync(ctx->d_masks[k], 0, ctx->masks_cap[k] * sizeof(uint32_t), ctx->stream));
+    const size_t cap_before = ctx->d_masks[k].cap;
+    CU(ctx->d_masks[k].grow(ctx->stream, (size_t)2 * P * MW + 16));
+    if (ctx->d_masks[k].cap != cap_before || ctx->masks_dirty) {
+      CU(cudaMemsetAsync(ctx->d_masks[k], 0, ctx->d_masks[k].cap * sizeof(uint32_t), ctx->stream));
       ctx->last_was_reduce = false;
     }
   }
   ctx->masks_dirty = false;
   uint32_t* const masks = ctx->d_masks[sset];
-  if ((rc = grow(ctx, &ctx->d_bits, &ctx->bits_cap, (size_t)3 * W + 2)) != GPR_OK) return rc;
-  if (comm && !fused &&
-      (rc = grow(ctx, &ctx->d_gather, &ctx->gather_cap, (size_t)ctx->world * 2 * W + 2)) != GPR_OK)
-    return rc;
+  CU(ctx->d_bits.grow(ctx->stream, (size_t)3 * W + 2));
+  if (comm && !fused) CU(ctx->d_gather.grow(ctx->stream, (size_t)ctx->world * 2 * W + 2));
   const bool want_smax = res->series_max != nullptr;
-  if (want_smax && host_out &&
-      (rc = grow(ctx, &ctx->d_smax, &ctx->smax_cap, (size_t)S + 4)) != GPR_OK)
-    return rc;
-  if (idle_slots && host_out && (rc = grow(ctx, &ctx->d_islots, &ctx->islots_cap, (size_t)P * MW + 4)) != GPR_OK)
-    return rc;
+  if (want_smax && host_out) CU(ctx->d_smax.grow(ctx->stream, (size_t)S + 4));
+  if (idle_slots && host_out) CU(ctx->d_islots.grow(ctx->stream, (size_t)P * MW + 4));
   if (grouped) {
-    if ((rc = grow(ctx, &ctx->d_grouped, &ctx->grouped_cap, (size_t)P * MW + 4)) != GPR_OK ||
-        (rc = grow(ctx, &ctx->d_gpods, &ctx->gpods_cap, (size_t)P + 4)) != GPR_OK ||
-        (!want_smax && (rc = grow(ctx, &ctx->d_gmax, &ctx->gmax_cap, (size_t)S + 4)) != GPR_OK) ||
-        (in_kind == GPR_MEM_HOST && (rc = grow(ctx, &ctx->d_gtable, &ctx->gtable_cap, (size_t)S + 4)) != GPR_OK))
-      return rc;
+    CU(ctx->d_grouped.grow(ctx->stream, (size_t)P * MW + 4));
+    CU(ctx->d_gpods.grow(ctx->stream, (size_t)P + 4));
+    if (!want_smax) CU(ctx->d_gmax.grow(ctx->stream, (size_t)S + 4));
+    if (in_kind == GPR_MEM_HOST) CU(ctx->d_gtable.grow(ctx->stream, (size_t)S + 4));
   }
 
   // ---- gates -----------------------------------------------------------------------------
   const uint8_t* d_elig = win->eligible;
   const int64_t* d_created = win->created_ts;
   if (gates_host && (win->eligible || win->created_ts)) {
-    if (P > ctx->gate_cap) {
-      if (ctx->d_elig_stage) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        CU(cudaFree(ctx->d_elig_stage));
-        CU(cudaFree(ctx->d_created_stage));
-        ctx->d_elig_stage = nullptr, ctx->d_created_stage = nullptr, ctx->gate_cap = 0;
-      }
-      const size_t cap = (size_t)P + P / 4 + 64;
-      CU(cudaMalloc(reinterpret_cast<void**>(&ctx->d_elig_stage), cap));
-      CU(cudaMalloc(reinterpret_cast<void**>(&ctx->d_created_stage), cap * sizeof(int64_t)));
-      ctx->gate_cap = cap;
-    }
+    CU(ctx->d_elig_stage.grow(ctx->stream, P));
+    CU(ctx->d_created_stage.grow(ctx->stream, P));
     ctx->last_was_reduce = false;
     if (win->eligible) {
       CU(cudaMemcpyAsync(ctx->d_elig_stage, win->eligible, P, cudaMemcpyHostToDevice, ctx->stream));
@@ -611,7 +617,7 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
       fp.peer_gather[r] = reinterpret_cast<uint32_t*>(ctx->p2p_peer[r] + ctx->p2p_gather_off[xset]);
       fp.peer_flag[r] = reinterpret_cast<unsigned long long*>(ctx->p2p_peer[r]) + ctx->rank;
     }
-    fp.my_flags = reinterpret_cast<const unsigned long long*>(ctx->p2p_block);
+    fp.my_flags = reinterpret_cast<const unsigned long long*>(ctx->p2p_block.p);
     if (ctx->exchange_ll) {
       for (int r = 0; r < ctx->world; ++r)
         fp.peer_ll[r] = reinterpret_cast<unsigned long long*>(ctx->p2p_peer[r] + ctx->p2p_ll_off[xset]);
@@ -723,7 +729,7 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
     rp.util_u8 = u8 ? 1u : 0u;
     const bool tma_ok = (T % 4u) == 0;
     const char* util_bytes = reinterpret_cast<const char*>(util);
-    char* stage_bytes = reinterpret_cast<char*>(ctx->d_util_stage);
+    char* stage_bytes = reinterpret_cast<char*>(ctx->d_util_stage.p);
     if (grouped && (rc = launch_group_rows()) != GPR_OK) return rc;
     for (uint32_t c = 0; c < n_chunks; ++c) {
       const uint32_t p0 = c * chunk_pods, p1 = std::min(P, p0 + chunk_pods);
@@ -1012,10 +1018,9 @@ int text_destination(gpr_ctx* ctx, const gpr_text_grid* grid, int32_t plane, gpr
     g->col_end = (ctx->res_head + ctx->res_T - 1) % ctx->res_T;  // the newest bucket sits just before the head
   } else {
     const size_t cells = (size_t)n_rows * n_samples;
-    const size_t cap_before = ctx->tplane_cap[plane];
-    int rc;
-    if ((rc = grow(ctx, &ctx->d_tplane[plane], &ctx->tplane_cap[plane], cells + 4)) != GPR_OK) return rc;
-    if (ctx->tplane_cap[plane] != cap_before && !(grid->flags & GPR_TEXT_FILL))
+    const size_t cap_before = ctx->d_tplane[plane].cap;
+    CU(ctx->d_tplane[plane].grow(ctx->stream, cells + 4));
+    if (ctx->d_tplane[plane].cap != cap_before && !(grid->flags & GPR_TEXT_FILL))
       return fail(ctx, GPR_E_STATE, "plane %d had to grow: the first parse of a window must pass GPR_TEXT_FILL", plane);
     *pl = ctx->d_tplane[plane];
     g->ld = n_samples, g->col_end = n_samples - 1;
@@ -1063,48 +1068,16 @@ int gpr_version(void) {
 
 const char* gpr_last_error(const gpr_ctx* ctx) { return ctx ? ctx->err : g_create_err; }
 
+// The members release every buffer, event and stream when ctx is deleted; this stops what could still use them first:
+// an unfinished scan's producer threads (joined, their streams drained), then the work on the context's stream.
 void gpr_destroy(gpr_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
+  scan_pipe_abort(ctx);
   if (ctx->stream) cudaStreamSynchronize(ctx->stream);
   if (ctx->comm && g_nccl.ok) g_nccl.CommDestroy(ctx->comm);
   for (int r = 0; r < gpr::kMaxPeers; ++r)
     if (ctx->p2p_peer[r] && ctx->p2p_peer[r] != ctx->p2p_block) cudaIpcCloseMemHandle(ctx->p2p_peer[r]);
-  if (ctx->p2p_block) cudaFree(ctx->p2p_block);
-  void* dev[] = {ctx->d_util_stage, ctx->d_power_stage, ctx->d_elig_stage, ctx->d_created_stage,
-                 ctx->d_masks[0],   ctx->d_masks[1],    ctx->d_bits,       ctx->d_gather,
-                 ctx->d_smax,       ctx->d_acc,         ctx->d_tickets,    ctx->d_done,
-                 ctx->d_flush,      ctx->d_res_util,    ctx->d_res_power,  ctx->d_cols,
-                 ctx->d_idx_util,   ctx->d_idx_power,   ctx->d_text[0],    ctx->d_text[1],
-                 ctx->d_text[2],    ctx->d_marks,       ctx->d_mark_counts, ctx->d_spans,
-                 ctx->d_tplane[0],  ctx->d_tplane[1],  ctx->d_grouped,   ctx->d_gpods,
-                 ctx->d_gmax,       ctx->d_gtable,     ctx->d_islots,    ctx->d_soffsets,
-                 ctx->d_srows,      ctx->d_sstats,     ctx->d_sstage};
-  for (void* p : dev)
-    if (p) cudaFree(p);
-  if (ctx->h_counts) cudaFreeHost(ctx->h_counts);
-  if (ctx->h_sstage) cudaFreeHost(ctx->h_sstage);
-  for (int b = 0; b < 2; ++b) {
-    if (ctx->ev_sup[b]) cudaEventDestroy(ctx->ev_sup[b]);
-    if (ctx->ev_sdone[b]) cudaEventDestroy(ctx->ev_sdone[b]);
-  }
-  scan_pipe_abort(ctx);
-  if (ctx->h_up_ring) cudaFreeHost(ctx->h_up_ring);
-  if (ctx->h_mark_blocks) cudaFreeHost(ctx->h_mark_blocks);
-  if (ctx->d_mark_blocks) cudaFree(ctx->d_mark_blocks);
-  for (cudaEvent_t e : ctx->mark_event)
-    if (e) cudaEventDestroy(e);
-  for (int k = 0; k < gpr_ctx::kUpThreads; ++k) {
-    if (ctx->up_stream[k]) cudaStreamDestroy(ctx->up_stream[k]);
-    for (cudaEvent_t e : ctx->up_event[k])
-      if (e) cudaEventDestroy(e);
-  }
-  cudaEvent_t evs[] = {ctx->ev_k0, ctx->ev_k1, ctx->ev_t0, ctx->ev_t1, ctx->ev_join};
-  for (cudaEvent_t e : evs)
-    if (e) cudaEventDestroy(e);
-  for (cudaEvent_t e : ctx->ev_chunk)
-    if (e) cudaEventDestroy(e);
-  if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
   if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
   delete ctx;
 }
@@ -1155,16 +1128,13 @@ int gpr_create(const gpr_config* cfg, gpr_ctx** out) {
       CU(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
       c->own_stream = true;
     }
-    CU(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
-    CU(cudaEventCreate(&c->ev_k0));
-    CU(cudaEventCreate(&c->ev_k1));
-    CU(cudaEventCreate(&c->ev_t0));
-    CU(cudaEventCreate(&c->ev_t1));
-    CU(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
-    for (cudaEvent_t& ev : c->ev_chunk) CU(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    CU(cudaMalloc(reinterpret_cast<void**>(&c->d_acc), 6 * sizeof(unsigned long long)));
-    CU(cudaMalloc(reinterpret_cast<void**>(&c->d_tickets), 2 * sizeof(unsigned int)));
-    CU(cudaMalloc(reinterpret_cast<void**>(&c->d_done), 2 * sizeof(unsigned long long)));
+    CU(c->copy_stream.create(cudaStreamNonBlocking));
+    for (Event* ev : {&c->ev_k0, &c->ev_k1, &c->ev_t0, &c->ev_t1}) CU(ev->create(cudaEventDefault));
+    CU(c->ev_join.create(cudaEventDisableTiming));
+    for (Event& ev : c->ev_chunk) CU(ev.create(cudaEventDisableTiming));
+    CU(c->d_acc.alloc(6));
+    CU(c->d_tickets.alloc(2));
+    CU(c->d_done.alloc(2));
     CU(cudaMemset(c->d_acc, 0, 6 * sizeof(unsigned long long)));
     CU(cudaMemset(c->d_tickets, 0, 2 * sizeof(unsigned int)));
     CU(cudaMemset(c->d_done, 0, 2 * sizeof(unsigned long long)));
@@ -1180,9 +1150,8 @@ int gpr_create(const gpr_config* cfg, gpr_ctx** out) {
     }
     c->fold_threads = env_int("GPR_FOLD_THREADS", 256);
     if (c->fold_threads != 64 && c->fold_threads != 128 && c->fold_threads != 256) c->fold_threads = 256;
-    CU(cudaMallocHost(reinterpret_cast<void**>(&c->h_counts),
-                      ((size_t)kSlots * 8 + 2) * sizeof(unsigned long long)));
-    memset(c->h_counts, 0, ((size_t)kSlots * 8 + 2) * sizeof(unsigned long long));
+    CU(c->h_counts.alloc((size_t)kSlots * 8 + 2));
+    memset(c->h_counts, 0, c->h_counts.cap * sizeof(unsigned long long));
     c->h_mark = c->h_counts + (size_t)kSlots * 8;
     c->h_err = reinterpret_cast<unsigned int*>(c->h_mark + 1);
     c->h_gerr = c->h_err + 1;
@@ -1228,9 +1197,8 @@ int gpr_create(const gpr_config* cfg, gpr_ctx** out) {
     c->cap_power = (cfg->flags & GPR_F_POWER_PLANE) != 0;
     const size_t cells = (size_t)cfg->max_pods * cfg->max_gpus * cfg->max_samples;
     if (cells) {
-      CU(cudaMalloc(reinterpret_cast<void**>(&c->d_util_stage), cells * sizeof(float) + 256));
-      if (c->cap_power)
-        CU(cudaMalloc(reinterpret_cast<void**>(&c->d_power_stage), cells * sizeof(float) + 256));
+      CU(c->d_util_stage.alloc(cells + 64));
+      if (c->cap_power) CU(c->d_power_stage.alloc(cells + 64));
     }
     return GPR_OK;
   };
@@ -1307,28 +1275,24 @@ int gpr_resident_init(gpr_ctx* ctx, uint32_t P, uint32_t G, uint32_t T, uint32_t
   if ((uint64_t)P * G > 0x7fffffffull) return fail(ctx, GPR_E_INVALID, "too many series");
   CU(cudaSetDevice(ctx->device));
   CU(cudaStreamSynchronize(ctx->stream));
-  if (ctx->d_res_util) CU(cudaFree(ctx->d_res_util));
-  if (ctx->d_res_power) CU(cudaFree(ctx->d_res_power));
-  ctx->d_res_util = ctx->d_res_power = nullptr;
-  const size_t bytes = (size_t)P * G * T * sizeof(float);
-  CU(cudaMalloc(reinterpret_cast<void**>(&ctx->d_res_util), bytes));
+  for (Buf<float>* b : {&ctx->d_res_util, &ctx->d_res_power, &ctx->d_idx_util, &ctx->d_idx_power}) CU(b->release());
+  ctx->idx_ld = 0;
+  const size_t cells = (size_t)P * G * T;
+  CU(ctx->d_res_util.alloc(cells));
   // 0xFFFFFFFF is a NaN: every step starts out "no sample"
-  CU(cudaMemsetAsync(ctx->d_res_util, 0xFF, bytes, ctx->stream));
+  CU(cudaMemsetAsync(ctx->d_res_util, 0xFF, cells * sizeof(float), ctx->stream));
   if (flags & GPR_F_POWER_PLANE) {
-    CU(cudaMalloc(reinterpret_cast<void**>(&ctx->d_res_power), bytes));
-    CU(cudaMemsetAsync(ctx->d_res_power, 0xFF, bytes, ctx->stream));
+    CU(ctx->d_res_power.alloc(cells));
+    CU(cudaMemsetAsync(ctx->d_res_power, 0xFF, cells * sizeof(float), ctx->stream));
   }
-  if (ctx->d_idx_util) CU(cudaFree(ctx->d_idx_util));
-  if (ctx->d_idx_power) CU(cudaFree(ctx->d_idx_power));
-  ctx->d_idx_util = ctx->d_idx_power = nullptr, ctx->idx_ld = 0;
   if (flags & GPR_F_BLOCK_INDEX) {
     ctx->idx_ld = gpr::index_ld(T);
-    const size_t ib = (size_t)P * G * ctx->idx_ld * sizeof(float);
-    CU(cudaMalloc(reinterpret_cast<void**>(&ctx->d_idx_util), ib));
-    CU(cudaMemsetAsync(ctx->d_idx_util, 0xFF, ib, ctx->stream));
+    const size_t ic = (size_t)P * G * ctx->idx_ld;
+    CU(ctx->d_idx_util.alloc(ic));
+    CU(cudaMemsetAsync(ctx->d_idx_util, 0xFF, ic * sizeof(float), ctx->stream));
     if (flags & GPR_F_POWER_PLANE) {
-      CU(cudaMalloc(reinterpret_cast<void**>(&ctx->d_idx_power), ib));
-      CU(cudaMemsetAsync(ctx->d_idx_power, 0xFF, ib, ctx->stream));
+      CU(ctx->d_idx_power.alloc(ic));
+      CU(cudaMemsetAsync(ctx->d_idx_power, 0xFF, ic * sizeof(float), ctx->stream));
     }
   }
   CU(cudaStreamSynchronize(ctx->stream));
@@ -1395,8 +1359,7 @@ int gpr_append(gpr_ctx* ctx, const float* util_cols, const float* power_cols, ui
     const float* src = planes_in[pl] + sp.src_col;
     uint64_t ld_dev = ld;
     if (mem_kind == GPR_MEM_HOST) {
-      int rc = grow(ctx, &ctx->d_cols, &ctx->cols_cap, rows * n_eff + 4);
-      if (rc != GPR_OK) return rc;
+      CU(ctx->d_cols.grow(ctx->stream, rows * n_eff + 4));
       if (ld == n_eff)  // dense block: one linear copy (a 2-D copy of 720-byte rows runs at ~6 GB/s)
         CU(cudaMemcpyAsync(ctx->d_cols, src, rows * (size_t)n_eff * 4u, cudaMemcpyHostToDevice,
                            ctx->stream));
@@ -1538,7 +1501,7 @@ int gpr_p2p_init(gpr_ctx* ctx, int rank, int world, uint32_t max_pods_per_rank, 
     ctx->p2p_ll_off[k] = 256 + (size_t)kExchangeDepth * gather_bytes + (size_t)k * ll_bytes;
   }
   const size_t total = 256 + (size_t)kExchangeDepth * (gather_bytes + ll_bytes);
-  CU(cudaMalloc(reinterpret_cast<void**>(&ctx->p2p_block), total));
+  CU(ctx->p2p_block.alloc(total));
   CU(cudaMemset(ctx->p2p_block, 0, total));
   cudaIpcMemHandle_t h;
   CU(cudaIpcGetMemHandle(&h, ctx->p2p_block));
@@ -1627,13 +1590,11 @@ int gpr_timer_begin(gpr_ctx* ctx) {
     q.seq = ++ctx->rdv_seq;
     for (int r = 0; r < ctx->world; ++r)
       q.peer_flag[r] = reinterpret_cast<unsigned long long*>(ctx->p2p_peer[r]) + gpr::kMaxPeers + ctx->rank;
-    q.my_flags = reinterpret_cast<const unsigned long long*>(ctx->p2p_block) + gpr::kMaxPeers;
+    q.my_flags = reinterpret_cast<const unsigned long long*>(ctx->p2p_block.p) + gpr::kMaxPeers;
   } else if (ctx->comm && ctx->world > 1) {
     // NCCL only: a one-word allgather is the rendezvous
-    int rc = grow(ctx, &ctx->d_gather, &ctx->gather_cap, (size_t)ctx->world + 2);
-    if (rc != GPR_OK) return rc;
-    rc = grow(ctx, &ctx->d_bits, &ctx->bits_cap, 4);
-    if (rc != GPR_OK) return rc;
+    CU(ctx->d_gather.grow(ctx->stream, (size_t)ctx->world + 2));
+    CU(ctx->d_bits.grow(ctx->stream, 4));
     NC(g_nccl.AllGather(ctx->d_bits, ctx->d_gather, 1, ncclUint32, ctx->comm, ctx->stream));
   }
   gpr::k_rendezvous<<<1, 32, 0, ctx->stream>>>(q);
@@ -1678,11 +1639,8 @@ int gpr_flush_l2(gpr_ctx* ctx) {
   if (!ctx) return GPR_E_INVALID;
   ctx->last_was_reduce = false;
   CU(cudaSetDevice(ctx->device));
-  if (!ctx->d_flush) {
-    ctx->flush_bytes = std::max<size_t>(ctx->l2_bytes * 2, (size_t)256 << 20);
-    CU(cudaMalloc(&ctx->d_flush, ctx->flush_bytes));
-  }
-  CU(cudaMemsetAsync(ctx->d_flush, 0x5a, ctx->flush_bytes, ctx->stream));
+  CU(ctx->d_flush.alloc_once(std::max<size_t>(ctx->l2_bytes * 2, (size_t)256 << 20)));
+  CU(cudaMemsetAsync(ctx->d_flush, 0x5a, ctx->d_flush.cap, ctx->stream));
   return GPR_OK;
 }
 int gpr_launch_count(const gpr_ctx* ctx, uint64_t* n) {
@@ -1717,19 +1675,14 @@ int gpr_text_scan_begin(gpr_ctx* ctx, int32_t slot, const char* text, uint64_t n
   if (mem_kind != GPR_MEM_HOST && mem_kind != GPR_MEM_DEVICE) return fail(ctx, GPR_E_INVALID, "bad mem_kind %d", mem_kind);
   scan_pipe_abort(ctx);  // an unfinished scan is dropped
   CU(cudaSetDevice(ctx->device));
-  int rc;
-  if ((rc = grow(ctx, &ctx->d_text[slot], &ctx->text_cap[slot], (size_t)n_bytes + gpr::text::kTextPad)) != GPR_OK)
-    return rc;
+  CU(ctx->d_text[slot].grow(ctx->stream, (size_t)n_bytes + gpr::text::kTextPad));
   constexpr int NT = gpr_ctx::kUpThreads, NS = gpr_ctx::kUpSlots, NB = gpr_ctx::kMarkBlocks;
-  if (!ctx->h_mark_blocks) {
-    CU(cudaHostAlloc(reinterpret_cast<void**>(&ctx->h_mark_blocks), (size_t)NB * kBlockWords * sizeof(uint32_t),
-                     cudaHostAllocMapped));
-    CU(cudaMalloc(reinterpret_cast<void**>(&ctx->d_mark_blocks), (size_t)NB * kBlockWords * sizeof(uint32_t)));
-    for (int b = 0; b < NB; ++b) CU(cudaEventCreateWithFlags(&ctx->mark_event[b], cudaEventDisableTiming));
-    for (int k = 0; k < NT; ++k) {
-      CU(cudaStreamCreateWithFlags(&ctx->up_stream[k], cudaStreamNonBlocking));
-      for (int s = 0; s < NS; ++s) CU(cudaEventCreateWithFlags(&ctx->up_event[k][s], cudaEventDisableTiming));
-    }
+  CU(ctx->h_mark_blocks.alloc_once((size_t)NB * kBlockWords, cudaHostAllocMapped));
+  CU(ctx->d_mark_blocks.alloc_once((size_t)NB * kBlockWords));
+  for (Event& ev : ctx->mark_event) CU(ev.create(cudaEventDisableTiming));
+  for (int k = 0; k < NT; ++k) {
+    CU(ctx->up_stream[k].create(cudaStreamNonBlocking));
+    for (Event& ev : ctx->up_event[k]) CU(ev.create(cudaEventDisableTiming));
   }
   uint8_t* d = ctx->d_text[slot];
   ctx->text_n[slot] = n_bytes;
@@ -1756,9 +1709,7 @@ int gpr_text_scan_begin(gpr_ctx* ctx, int32_t slot, const char* text, uint64_t n
   static_assert(gpr_ctx::kPinnedChunk / gpr_ctx::kScanUnit <= (size_t)gpr_ctx::kMarkBlocks, "a chunk's units fit the ring");
   // pinned and device sources need no staging copy: one producer keeps the DMA engine busy
   sp->nt = sp->staged ? (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)ctx->up_threads, sp->n_chunks)) : 1;
-  if (sp->staged && !ctx->h_up_ring)
-    CU(cudaHostAlloc(reinterpret_cast<void**>(&ctx->h_up_ring), (size_t)ctx->up_threads * NS * ctx->up_slot_bytes,
-                     cudaHostAllocDefault));
+  if (sp->staged) CU(ctx->h_up_ring.alloc_once((size_t)ctx->up_threads * NS * ctx->up_slot_bytes));
   ctx->pipe = sp;
   ctx->launches += 2 * sp->n_chunks;
   try {
@@ -1887,7 +1838,7 @@ int gpr_text_parse(gpr_ctx* ctx, int32_t slot, gpr_text_span* spans, uint32_t n_
   gpr::text::Grid g;
   if ((rc = text_destination(ctx, grid, plane, &g, &pl)) != GPR_OK) return rc;
   if ((rc = open_destination(ctx, grid, pl)) != GPR_OK) return rc;
-  if ((rc = grow(ctx, &ctx->d_spans, &ctx->spans_cap, (size_t)n_spans + 1)) != GPR_OK) return rc;
+  CU(ctx->d_spans.grow(ctx->stream, (size_t)n_spans + 1));
   ctx->last_was_reduce = false;
   if (n_spans && n) {
     CU(cudaMemcpyAsync(ctx->d_spans, spans, (size_t)n_spans * sizeof(gpr_text_span), cudaMemcpyHostToDevice,
@@ -1933,9 +1884,8 @@ static int launch_scatter(gpr_ctx* ctx, const gpr::samples::ScatterArgs& a, bool
 static int scatter_host_pieces(gpr_ctx* ctx, const gpr_sample_batch* batch, uint64_t total, gpr::samples::ScatterArgs a) {
   namespace gs = gpr::samples;
   const uint32_t S = batch->n_series;
-  int rc;
-  if ((rc = grow(ctx, &ctx->d_soffsets, &ctx->soffsets_cap, (size_t)S + 1)) != GPR_OK) return rc;
-  if ((rc = grow(ctx, &ctx->d_srows, &ctx->srows_cap, (size_t)S + 1)) != GPR_OK) return rc;
+  CU(ctx->d_soffsets.grow(ctx->stream, (size_t)S + 1));
+  CU(ctx->d_srows.grow(ctx->stream, (size_t)S + 1));
   CU(cudaMemcpyAsync(ctx->d_soffsets, batch->offsets, ((size_t)S + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaMemcpyAsync(ctx->d_srows, batch->rows, (size_t)S * 4, cudaMemcpyHostToDevice, ctx->stream));
   a.offsets = ctx->d_soffsets, a.rows = ctx->d_srows;
@@ -1946,11 +1896,11 @@ static int scatter_host_pieces(gpr_ctx* ctx, const gpr_sample_batch* batch, uint
     (void)cudaGetLastError();  // an unregistered pointer may leave an error code behind
   }
   const size_t half = gs::kHostPiece * 8;  // bytes of one piece's timestamps, or of its values
-  if (!ctx->d_sstage) CU(cudaMalloc(reinterpret_cast<void**>(&ctx->d_sstage), 4 * half));
-  if (!pinned && !ctx->h_sstage) CU(cudaMallocHost(reinterpret_cast<void**>(&ctx->h_sstage), 4 * half));
+  CU(ctx->d_sstage.alloc_once(4 * half));
+  if (!pinned) CU(ctx->h_sstage.alloc_once(4 * half));
   for (int b = 0; b < 2; ++b) {
-    if (!ctx->ev_sup[b]) CU(cudaEventCreateWithFlags(&ctx->ev_sup[b], cudaEventDisableTiming));
-    if (!ctx->ev_sdone[b]) CU(cudaEventCreateWithFlags(&ctx->ev_sdone[b], cudaEventDisableTiming));
+    CU(ctx->ev_sup[b].create(cudaEventDisableTiming));
+    CU(ctx->ev_sdone[b].create(cudaEventDisableTiming));
   }
   uint64_t k = 0;
   return gs::for_each_piece(batch->offsets, S, total, gs::kHostPiece, [&](const gs::Piece& p) -> int {
@@ -2000,7 +1950,7 @@ int gpr_samples_scatter(gpr_ctx* ctx, const gpr_sample_batch* batch, const gpr_t
   if (!batch->offsets || (S && !batch->rows)) return fail(ctx, GPR_E_INVALID, "offsets / rows is NULL");
   CU(cudaSetDevice(ctx->device));
   ctx->last_was_reduce = false;
-  if (!ctx->d_sstats) CU(cudaMalloc(reinterpret_cast<void**>(&ctx->d_sstats), 4 * sizeof(unsigned long long)));
+  CU(ctx->d_sstats.alloc_once(4));
   // ---- the batch is checked before anything is written
   uint32_t bad = 0;
   uint64_t total = 0;

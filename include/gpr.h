@@ -226,6 +226,8 @@ typedef struct gpr_result {
 /* ---- lifecycle ----------------------------------------------------------------------- */
 GPR_API int gpr_version(void); /* major*10000 + minor*100 + patch */
 GPR_API int gpr_create(const gpr_config *cfg, gpr_ctx **out);
+/* Releases everything the context owns.  An unfinished gpr_text_scan_begin is stopped (its upload threads joined,
+ * their copies and scans drained) and the context's stream synchronised before anything is released. */
 GPR_API void gpr_destroy(gpr_ctx *ctx);
 GPR_API const char *gpr_last_error(const gpr_ctx *ctx);
 
