@@ -32,6 +32,7 @@
 #include "gpr_synth.cuh"
 #include "gpr_text_kernels.cuh"
 #include "gpr_samples.cuh"
+#include "gpr_chunks.cuh"
 
 namespace {
 
@@ -266,6 +267,9 @@ struct gpr_ctx {
   PinnedBuf<unsigned char> h_sstage;   // the same, pinned
   Event ev_sup[2];                     // piece in buffer b uploaded
   Event ev_sdone[2];                   // piece in buffer b scattered
+  // XOR chunks (gpr_chunks_scatter) share that staging, and d_soffsets / d_srows for a host batch's series_chunks
+  // and rows
+  Buf<uint64_t> d_cbytes;              // a host batch's chunk_bytes, uploaded whole (8 B per chunk)
 
   // multi-GPU
   ncclComm_t comm = nullptr;
@@ -1879,8 +1883,68 @@ static int launch_scatter(gpr_ctx* ctx, const gpr::samples::ScatterArgs& a, bool
   return GPR_OK;
 }
 
-// A host batch, piece by piece: piece k is copied (through pinned staging if the batch is pageable) into device buffer
-// k % 2 on the copy stream and scattered on the context's stream, so piece k + 1 crosses PCIe while piece k merges.
+// Whether both host arrays are pinned (registered with CUDA); pageable ones go up through pinned staging.
+static bool host_pinned(const void* a, const void* b) {
+  bool pinned = true;
+  for (const void* p : {a, b}) {
+    if (!p) continue;
+    cudaPointerAttributes at;
+    pinned = pinned && cudaPointerGetAttributes(&at, p) == cudaSuccess && at.type == cudaMemoryTypeHost;
+    (void)cudaGetLastError();  // an unregistered pointer may leave an error code behind
+  }
+  return pinned;
+}
+
+// The staging of a host batch (gpr_samples_scatter, gpr_chunks_scatter): two device buffers of 2 x kStageHalf bytes
+// and, for pageable batches, two pinned ones.  Piece k goes into buffer k % 2.
+constexpr size_t kStageHalf = gpr::samples::kHostPiece * 8;  // bytes of one piece's timestamps, or of its values
+static_assert(gpr::chunks::kHostPiece == 2 * kStageHalf, "a piece of chunk data fills one staging buffer");
+
+static int open_staging(gpr_ctx* ctx, bool pinned) {
+  CU(ctx->d_sstage.alloc_once(4 * kStageHalf));
+  if (!pinned) CU(ctx->h_sstage.alloc_once(4 * kStageHalf));
+  for (int b = 0; b < 2; ++b) {
+    CU(ctx->ev_sup[b].create(cudaEventDisableTiming));
+    CU(ctx->ev_sdone[b].create(cudaEventDisableTiming));
+  }
+  return GPR_OK;
+}
+
+// Piece k of a host batch: the host ranges src[i] (bytes[i] each, at most kStageHalf when there are two, or
+// 2 x kStageHalf for one) are copied, through pinned staging unless `pinned`, into device buffer k % 2 on the copy
+// stream; the context's stream waits for them and consume(device buffer) enqueues the work on the piece, after which
+// the buffer is marked free.  So piece k + 1 crosses PCIe while piece k is consumed.
+extern "C++" {  // (templates)
+template <typename Consume>
+static int stage_piece(gpr_ctx* ctx, uint64_t k, bool pinned, const void* const (&src)[2], const size_t (&bytes)[2],
+                       Consume&& consume) {
+  const int b = (int)(k & 1);
+  unsigned char* dst = ctx->d_sstage + (size_t)b * 2 * kStageHalf;
+  if (k >= 2) CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_sdone[b], 0));  // piece k - 2 has left buffer b
+  if (!pinned && k >= 2) CU(cudaEventSynchronize(ctx->ev_sup[b]));  // piece k - 2's upload has drained pinned buffer b
+  size_t at = 0;
+  for (int i = 0; i < 2; ++i) {
+    if (!bytes[i]) continue;
+    const void* from = src[i];
+    if (!pinned) {
+      unsigned char* stage = ctx->h_sstage + (size_t)b * 2 * kStageHalf + at;
+      memcpy(stage, src[i], bytes[i]);
+      from = stage;
+    }
+    CU(cudaMemcpyAsync(dst + at, from, bytes[i], cudaMemcpyHostToDevice, ctx->copy_stream));
+    at += kStageHalf;
+  }
+  CU(cudaEventRecord(ctx->ev_sup[b], ctx->copy_stream));
+  CU(cudaStreamWaitEvent(ctx->stream, ctx->ev_sup[b], 0));
+  const int r = consume(dst);
+  if (r != GPR_OK) return r;
+  CU(cudaEventRecord(ctx->ev_sdone[b], ctx->stream));
+  return GPR_OK;
+}
+}  // extern "C++"
+
+// A host batch, piece by piece: piece k is copied into device buffer k % 2 on the copy stream and scattered on the
+// context's stream, so piece k + 1 crosses PCIe while piece k merges.
 static int scatter_host_pieces(gpr_ctx* ctx, const gpr_sample_batch* batch, uint64_t total, gpr::samples::ScatterArgs a) {
   namespace gs = gpr::samples;
   const uint32_t S = batch->n_series;
@@ -1889,46 +1953,20 @@ static int scatter_host_pieces(gpr_ctx* ctx, const gpr_sample_batch* batch, uint
   CU(cudaMemcpyAsync(ctx->d_soffsets, batch->offsets, ((size_t)S + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
   CU(cudaMemcpyAsync(ctx->d_srows, batch->rows, (size_t)S * 4, cudaMemcpyHostToDevice, ctx->stream));
   a.offsets = ctx->d_soffsets, a.rows = ctx->d_srows;
-  bool pinned = true;
-  for (const void* p : {(const void*)batch->ts_ms, (const void*)batch->values}) {
-    cudaPointerAttributes at;
-    pinned = pinned && cudaPointerGetAttributes(&at, p) == cudaSuccess && at.type == cudaMemoryTypeHost;
-    (void)cudaGetLastError();  // an unregistered pointer may leave an error code behind
-  }
-  const size_t half = gs::kHostPiece * 8;  // bytes of one piece's timestamps, or of its values
-  CU(ctx->d_sstage.alloc_once(4 * half));
-  if (!pinned) CU(ctx->h_sstage.alloc_once(4 * half));
-  for (int b = 0; b < 2; ++b) {
-    CU(ctx->ev_sup[b].create(cudaEventDisableTiming));
-    CU(ctx->ev_sdone[b].create(cudaEventDisableTiming));
-  }
+  const bool pinned = host_pinned(batch->ts_ms, batch->values);
+  int rc;
+  if ((rc = open_staging(ctx, pinned)) != GPR_OK) return rc;
   uint64_t k = 0;
   return gs::for_each_piece(batch->offsets, S, total, gs::kHostPiece, [&](const gs::Piece& p) -> int {
-    const int b = (int)(k & 1);
     const uint64_t n = p.end - p.begin;
-    unsigned char* dst = ctx->d_sstage + (size_t)b * 2 * half;
-    const void* src_t = batch->ts_ms + p.begin;
-    const void* src_v = batch->values + p.begin;
-    if (k >= 2) CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_sdone[b], 0));  // piece k - 2 has left buffer b
-    if (!pinned) {
-      unsigned char* stage = ctx->h_sstage + (size_t)b * 2 * half;
-      if (k >= 2) CU(cudaEventSynchronize(ctx->ev_sup[b]));  // piece k - 2's upload has drained pinned buffer b
-      memcpy(stage, src_t, n * 8);
-      memcpy(stage + half, src_v, n * 8);
-      src_t = stage, src_v = stage + half;
-    }
-    CU(cudaMemcpyAsync(dst, src_t, n * 8, cudaMemcpyHostToDevice, ctx->copy_stream));
-    CU(cudaMemcpyAsync(dst + half, src_v, n * 8, cudaMemcpyHostToDevice, ctx->copy_stream));
-    CU(cudaEventRecord(ctx->ev_sup[b], ctx->copy_stream));
-    CU(cudaStreamWaitEvent(ctx->stream, ctx->ev_sup[b], 0));
-    a.ts = reinterpret_cast<const int64_t*>(dst);
-    a.values = reinterpret_cast<const double*>(dst + half);
-    a.base = p.begin, a.end = p.end, a.s_base = p.series;
-    const int r = launch_scatter(ctx, a, true);
-    if (r != GPR_OK) return r;
-    CU(cudaEventRecord(ctx->ev_sdone[b], ctx->stream));
-    ++k;
-    return GPR_OK;
+    const void* const src[2] = {batch->ts_ms + p.begin, batch->values + p.begin};
+    const size_t bytes[2] = {n * 8, n * 8};
+    return stage_piece(ctx, k++, pinned, src, bytes, [&](unsigned char* dst) {
+      a.ts = reinterpret_cast<const int64_t*>(dst);
+      a.values = reinterpret_cast<const double*>(dst + kStageHalf);
+      a.base = p.begin, a.end = p.end, a.s_base = p.series;
+      return launch_scatter(ctx, a, true);
+    });
   });
 }
 
@@ -1997,6 +2035,192 @@ int gpr_samples_scatter(gpr_ctx* ctx, const gpr_sample_batch* batch, const gpr_t
   CU(cudaMemcpyAsync(counts, ctx->d_sstats, sizeof counts, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   if (stats) stats->n_in = total, stats->n_oow = counts[0], stats->n_tiny = counts[1];
+  return GPR_OK;
+  GPR_CATCH(ctx)
+}
+
+// ---- Prometheus XOR chunks (gpr_chunks.cuh) -----------------------------------------------------------------
+constexpr uint32_t kChunkTooLarge = 1u << 31;  // a host batch's chunk that does not fit one upload piece
+// The fault bits of a chunk batch as GPR_E_INVALID; `first` is the first chunk at fault (the bits are those of all
+// faulty chunks: the message gives the first kind found).
+static int chunk_batch_fault(gpr_ctx* ctx, uint32_t bad, uint64_t first, uint32_t n_rows) {
+  namespace gc = gpr::chunks;
+  const unsigned long long c = first;
+  if (bad & gc::kBadStart) return fail(ctx, GPR_E_INVALID, "gpr_chunk_batch: series_chunks[0] != 0");
+  if (bad & gc::kBadOrder) return fail(ctx, GPR_E_INVALID, "gpr_chunk_batch: series_chunks decrease");
+  if (bad & gc::kBadRow) return fail(ctx, GPR_E_INVALID, "gpr_chunk_batch: a row >= grid.n_rows (%u)", n_rows);
+  if (bad & gc::kBadChunkStart) return fail(ctx, GPR_E_INVALID, "gpr_chunk_batch: chunk_bytes[0] != 0");
+  const char* what = (bad & gc::kBadChunkOrder) ? "chunk_bytes decrease"
+                     : (bad & gc::kShort)       ? "shorter than its 2-byte header"
+                     : (bad & gc::kOverrun)     ? "its samples run past its bytes"
+                     : (bad & gc::kNoWindow)    ? "a value reuses the XOR window before one was set"
+                     : (bad & gc::kBadVarint)   ? "a varint overflows 64 bits"
+                                                : "a host chunk larger than an upload piece (32 MB)";
+  return fail(ctx, GPR_E_INVALID, "gpr_chunk_batch: chunk %llu is the first malformed one (%s)", c, what);
+}
+
+static int launch_chunks_check(gpr_ctx* ctx, const gpr::chunks::CheckArgs& a) {
+  const uint32_t blocks = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((a.end - a.base + 255) / 256,
+                                                                            (uint64_t)ctx->sm_count * 8));
+  gpr::chunks::k_chunks_check<<<blocks, 256, 0, ctx->stream>>>(a);
+  ctx->launches++;
+  CU(cudaGetLastError());
+  return GPR_OK;
+}
+
+static int launch_chunks_scatter(gpr_ctx* ctx, const gpr::chunks::ScatterArgs& a) {
+  namespace gc = gpr::chunks;
+  if (a.end <= a.base) return GPR_OK;
+  const uint64_t groups = (a.end - a.base + 31) / 32;
+  const uint32_t blocks = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((groups + gc::kWarps - 1) / gc::kWarps,
+                                                                            (uint64_t)ctx->sm_count * 8));
+  gc::k_chunks_scatter<<<blocks, gc::kThreads, 0, ctx->stream>>>(a);
+  ctx->launches++;
+  CU(cudaGetLastError());
+  return GPR_OK;
+}
+
+// A host batch's chunk data, piece by piece: each piece is the most whole chunks that fit kHostPiece bytes, and at
+// least one (none is larger: the host check saw to it); consume(piece, device bytes of the piece) enqueues the work
+// on each.
+extern "C++" {  // (templates)
+template <typename Consume>
+static int chunk_pieces(gpr_ctx* ctx, const gpr_chunk_batch* batch, uint64_t n_chunks, bool pinned, Consume&& consume) {
+  namespace gc = gpr::chunks;
+  namespace gs = gpr::samples;
+  const uint64_t* cb = batch->chunk_bytes;
+  const auto cut = [&](uint64_t b) {
+    const uint64_t* e = std::upper_bound(cb + b + 1, cb + n_chunks + 1, cb[b] + gc::kHostPiece);
+    return std::max<uint64_t>(b + 1, (uint64_t)(e - cb) - 1);
+  };
+  uint64_t k = 0;
+  return gs::for_each_cut(batch->series_chunks, batch->n_series, n_chunks, cut, [&](const gs::Piece& p) -> int {
+    const void* const src[2] = {batch->data + cb[p.begin], nullptr};
+    const size_t bytes[2] = {(size_t)(cb[p.end] - cb[p.begin]), 0};
+    return stage_piece(ctx, k++, pinned, src, bytes, [&](unsigned char* dst) { return consume(p, dst); });
+  });
+}
+}  // extern "C++"
+
+int gpr_chunks_scatter(gpr_ctx* ctx, const gpr_chunk_batch* batch, const gpr_text_grid* grid, int32_t plane,
+                       gpr_sample_stats* stats) {
+  if (!ctx) return GPR_E_INVALID;
+  GPR_TRY
+  NvtxRange nvtx_range("gpr_chunks_scatter");
+  namespace gc = gpr::chunks;
+  namespace gs = gpr::samples;
+  if (!batch || batch->struct_size != sizeof(gpr_chunk_batch))
+    return fail(ctx, GPR_E_INVALID, "batch is NULL / struct_size mismatch");
+  if (!grid || grid->struct_size != sizeof(gpr_text_grid)) return fail(ctx, GPR_E_INVALID, "grid is NULL / struct_size mismatch");
+  if (plane < 0 || plane > 1) return fail(ctx, GPR_E_INVALID, "bad plane %d", plane);
+  if (batch->mem_kind != GPR_MEM_HOST && batch->mem_kind != GPR_MEM_DEVICE)
+    return fail(ctx, GPR_E_INVALID, "bad mem_kind %d", batch->mem_kind);
+  int rc;
+  if ((rc = check_grid(ctx, grid)) != GPR_OK) return rc;
+  const uint32_t S = batch->n_series;
+  if (!batch->series_chunks || !batch->chunk_bytes || (S && !batch->rows))
+    return fail(ctx, GPR_E_INVALID, "series_chunks / chunk_bytes / rows is NULL");
+  CU(cudaSetDevice(ctx->device));
+  ctx->last_was_reduce = false;
+  CU(ctx->d_sstats.grow(ctx->stream, 5));  // [n_oow, n_tiny, check word, n_in, first bad chunk]
+  unsigned int* d_bad = reinterpret_cast<unsigned int*>(ctx->d_sstats + 2);
+  const bool host = batch->mem_kind == GPR_MEM_HOST;
+  // ---- the batch is checked before anything is written: the index arrays, then the chunks' data
+  uint32_t bad = 0;
+  uint64_t n_chunks = 0, first = ~0ull;
+  if (host) {
+    for (uint32_t s = 0; s < std::max(S, 1u); ++s)
+      bad |= gs::series_faults(batch->series_chunks, batch->rows, S, s, grid->n_rows);
+    if (bad) return chunk_batch_fault(ctx, bad, 0, grid->n_rows);
+    n_chunks = batch->series_chunks[S];
+    if (batch->chunk_bytes[0] != 0) bad |= gc::kBadChunkStart;
+    for (uint64_t c = 0; c < n_chunks && !bad; ++c) {
+      bad = gc::bound_faults(batch->chunk_bytes, c);
+      if (!bad && batch->chunk_bytes[c + 1] - batch->chunk_bytes[c] > gc::kHostPiece) bad = kChunkTooLarge;
+      if (bad) first = c;
+    }
+    if (bad) return chunk_batch_fault(ctx, bad, first, grid->n_rows);
+  } else {
+    unsigned long long back[2] = {0, 0};  // the check word, series_chunks[n_series]
+    CU(cudaMemsetAsync(d_bad, 0, sizeof(unsigned long long), ctx->stream));
+    const uint32_t blocks = std::max(1u, std::min((std::max(S, 1u) + 255u) / 256u, (uint32_t)ctx->sm_count * 8u));
+    gs::k_samples_check<<<blocks, 256, 0, ctx->stream>>>(batch->series_chunks, batch->rows, S, grid->n_rows, d_bad);
+    ctx->launches++;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(&back[0], d_bad, sizeof back[0], cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(&back[1], batch->series_chunks + S, sizeof back[1], cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    bad = (uint32_t)back[0], n_chunks = back[1];
+    if (bad) return chunk_batch_fault(ctx, bad, 0, grid->n_rows);
+  }
+  if (n_chunks && !batch->data) return fail(ctx, GPR_E_INVALID, "data is NULL");
+  // the chunks' data, by the check kernel: in place for a device batch, piece by piece as it lands for a host one
+  CU(cudaMemsetAsync(ctx->d_sstats + 2, 0, 2 * sizeof(unsigned long long), ctx->stream));
+  CU(cudaMemsetAsync(ctx->d_sstats + 4, 0xFF, sizeof(unsigned long long), ctx->stream));
+  gc::CheckArgs ck;
+  ck.bad = d_bad, ck.n_in = ctx->d_sstats + 3, ck.first = ctx->d_sstats + 4;
+  const bool pinned = host && host_pinned(batch->data, nullptr);
+  std::vector<gs::Piece> checked;  // a host batch's pieces, in the order they went up
+  if (host) {
+    CU(ctx->d_soffsets.grow(ctx->stream, (size_t)S + 1));
+    CU(ctx->d_srows.grow(ctx->stream, (size_t)S + 1));
+    CU(ctx->d_cbytes.grow(ctx->stream, (size_t)n_chunks + 1));
+    CU(cudaMemcpyAsync(ctx->d_soffsets, batch->series_chunks, ((size_t)S + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemcpyAsync(ctx->d_srows, batch->rows, (size_t)S * 4, cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemcpyAsync(ctx->d_cbytes, batch->chunk_bytes, ((size_t)n_chunks + 1) * 8, cudaMemcpyHostToDevice,
+                       ctx->stream));
+    if ((rc = open_staging(ctx, pinned)) != GPR_OK) return rc;
+    rc = chunk_pieces(ctx, batch, n_chunks, pinned, [&](const gs::Piece& p, const unsigned char* d) {
+      checked.push_back(p);
+      ck.chunk_bytes = ctx->d_cbytes, ck.data = d, ck.data_base = batch->chunk_bytes[p.begin];
+      ck.base = p.begin, ck.end = p.end;
+      return launch_chunks_check(ctx, ck);
+    });
+  } else {
+    ck.chunk_bytes = batch->chunk_bytes, ck.data = batch->data, ck.data_base = 0, ck.base = 0, ck.end = n_chunks;
+    rc = launch_chunks_check(ctx, ck);
+  }
+  if (rc != GPR_OK) {
+    (void)cudaStreamSynchronize(ctx->stream);  // the staging buffers may still be read
+    return rc;
+  }
+  unsigned long long back[3] = {0, 0, 0};  // the check word, n_in, the first bad chunk
+  CU(cudaMemcpyAsync(back, ctx->d_sstats + 2, sizeof back, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  if (back[0]) return chunk_batch_fault(ctx, (uint32_t)back[0], back[2], grid->n_rows);
+  // ---- the destination, then the merge
+  float* pl = nullptr;
+  gc::ScatterArgs a;
+  memset(&a, 0, sizeof a);
+  if ((rc = text_destination(ctx, grid, plane, &a.g, &pl)) != GPR_OK) return rc;
+  if ((rc = open_destination(ctx, grid, pl)) != GPR_OK) return rc;
+  CU(cudaMemsetAsync(ctx->d_sstats, 0, 2 * sizeof(unsigned long long), ctx->stream));
+  a.n_series = S, a.plane = pl, a.stats = ctx->d_sstats;
+  if (!host) {  // read in place
+    a.series_chunks = batch->series_chunks, a.rows = batch->rows, a.chunk_bytes = batch->chunk_bytes;
+    a.data = batch->data, a.data_base = 0, a.base = 0, a.end = n_chunks, a.s_base = 0;
+    rc = launch_chunks_scatter(ctx, a);
+  } else {
+    a.series_chunks = ctx->d_soffsets, a.rows = ctx->d_srows, a.chunk_bytes = ctx->d_cbytes;
+    const auto scatter = [&](const gs::Piece& p, const unsigned char* d) {
+      a.data = d, a.data_base = batch->chunk_bytes[p.begin], a.base = p.begin, a.end = p.end, a.s_base = p.series;
+      return launch_chunks_scatter(ctx, a);
+    };
+    if (checked.size() <= 2) {  // the checked pieces are still in the two staging buffers
+      for (size_t k = 0; k < checked.size() && rc == GPR_OK; ++k)
+        rc = scatter(checked[k], ctx->d_sstage + k * 2 * kStageHalf);
+    } else {
+      rc = chunk_pieces(ctx, batch, n_chunks, pinned, scatter);
+    }
+  }
+  if (rc != GPR_OK) {
+    (void)cudaStreamSynchronize(ctx->stream);  // the staging buffers may still be read
+    return rc;
+  }
+  unsigned long long counts[2] = {0, 0};
+  CU(cudaMemcpyAsync(counts, ctx->d_sstats, sizeof counts, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  if (stats) stats->n_in = back[1], stats->n_oow = counts[0], stats->n_tiny = counts[1];
   return GPR_OK;
   GPR_CATCH(ctx)
 }

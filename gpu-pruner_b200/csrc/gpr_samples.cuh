@@ -71,19 +71,27 @@ struct Piece {
   uint32_t series;
 };
 
-// Cuts the samples [0, total) of a batch into pieces of at most `piece` samples, in order, wherever the cut falls:
-// between series or inside one.  fn(const Piece&) returns 0 to go on; the first other value stops the walk and is
-// returned.
-template <typename Fn>
-inline int for_each_piece(const uint64_t* offsets, uint32_t n_series, uint64_t total, uint64_t piece, Fn&& fn) {
+// Cuts the elements [0, total) of a CSR batch (samples here, chunks in gpr_chunks.cuh) into pieces, in order: the
+// piece that begins at b ends at cut(b), which must lie in (b, total].  fn(const Piece&) returns 0 to go on; the first
+// other value stops the walk and is returned.
+template <typename Cut, typename Fn>
+inline int for_each_cut(const uint64_t* offsets, uint32_t n_series, uint64_t total, Cut&& cut, Fn&& fn) {
   uint32_t s = 0;
-  for (uint64_t b = 0; b < total; b += piece) {
+  for (uint64_t b = 0; b < total;) {
     s = series_from(offsets, n_series, s, b);
-    const Piece p{b, total - b < piece ? total : b + piece, s};
+    const Piece p{b, cut(b), s};
     const int rc = fn(p);
     if (rc != 0) return rc;
+    b = p.end;
   }
   return 0;
+}
+
+// Cuts the samples [0, total) of a batch into pieces of at most `piece` samples, wherever the cut falls: between
+// series or inside one.
+template <typename Fn>
+inline int for_each_piece(const uint64_t* offsets, uint32_t n_series, uint64_t total, uint64_t piece, Fn&& fn) {
+  return for_each_cut(offsets, n_series, total, [&](uint64_t b) { return total - b < piece ? total : b + piece; }, fn);
 }
 
 struct ScatterArgs {
@@ -100,15 +108,15 @@ struct ScatterArgs {
 };
 
 // One sample: the cell and the value gpr_text_parse gives the same sample written as text.
-__device__ __forceinline__ void scatter_sample(const ScatterArgs& a, uint32_t row, int64_t ts, double v, uint32_t& n_oow,
-                           uint32_t& n_tiny) {
-  const int64_t col = text::column_of(a.g, ts);
+__device__ __forceinline__ void scatter_sample(const text::Grid& g, float* plane, uint32_t row, int64_t ts, double v,
+                                               uint32_t& n_oow, uint32_t& n_tiny) {
+  const int64_t col = text::column_of(g, ts);
   if (col < 0) {
     ++n_oow;
     return;
   }
-  const float f = text::snap_power(v, text::to_f32(v, &n_tiny), a.g.power);
-  text::atomic_merge(a.plane + (uint64_t)row * a.g.ld + (uint64_t)col, f);
+  const float f = text::snap_power(v, text::to_f32(v, &n_tiny), g.power);
+  text::atomic_merge(plane + (uint64_t)row * g.ld + (uint64_t)col, f);
 }
 
 // kVec: ts and values are 16-byte aligned, so a pair (i - base even) is one 128-bit load of each
@@ -154,7 +162,7 @@ __global__ void __launch_bounds__(kThreads) k_samples_scatter(const ScatterArgs 
         const uint64_t i = i0[k] + h;
         if (i >= a.end) break;
         s = series_from(a.offsets, a.n_series, s, i);
-        scatter_sample(a, __ldg(a.rows + s), t[k][h], v[k][h], n_oow, n_tiny);
+        scatter_sample(a.g, a.plane, __ldg(a.rows + s), t[k][h], v[k][h], n_oow, n_tiny);
       }
     }
   }

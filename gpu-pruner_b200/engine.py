@@ -470,6 +470,42 @@ class IdleEngine:
         self._check(self._lib.gpr_samples_scatter(self._h, C.byref(b), C.byref(g), plane, C.byref(st)))
         return {"n_in": st.n_in, "n_oow": st.n_oow, "n_tiny": st.n_tiny}
 
+    def chunks_scatter(self, series_chunks, rows, chunk_bytes, data, t_end: int, step: int, T: int, n_rows: int, *,
+                       window_seconds: Optional[int] = None, plane: int = 0, resident: bool = False,
+                       fill: bool = True, power_threshold: Optional[float] = 0.0, mem_kind: int = ffi.GPR_MEM_HOST,
+                       n_series: Optional[int] = None) -> dict:
+        """Decode Prometheus XOR chunks and merge their samples into the context's plane (or, ``resident=True``, the
+        resident ring), exactly as :meth:`samples_scatter` merges the same decoded samples.  CSR over chunks: series
+        s owns chunks ``series_chunks[s]:series_chunks[s+1]`` (uint64) and feeds row ``rows[s]`` (uint32); chunk c is
+        ``data[chunk_bytes[c]:chunk_bytes[c+1]]`` (uint64 offsets into the uint8 ``data``).  Host arrays (numpy) are
+        converted to those dtypes; with ``mem_kind=GPR_MEM_DEVICE`` pass device addresses / tensors and
+        ``n_series``.  Returns the counts ``{"n_in", "n_oow", "n_tiny"}``."""
+        if mem_kind == ffi.GPR_MEM_HOST:
+            series_chunks = np.ascontiguousarray(series_chunks, dtype=np.uint64)
+            rows = np.ascontiguousarray(rows, dtype=np.uint32)
+            chunk_bytes = np.ascontiguousarray(chunk_bytes, dtype=np.uint64)
+            data = np.ascontiguousarray(np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray))
+                                        else data, dtype=np.uint8)
+            if n_series is None:
+                n_series = rows.size
+        elif n_series is None:
+            raise ValueError("n_series is required for device arrays")
+        b = ffi.gpr_chunk_batch()
+        b.struct_size = C.sizeof(ffi.gpr_chunk_batch)
+        b.mem_kind = mem_kind
+        b.series_chunks, b.rows, b.chunk_bytes, b.data = _ptr(series_chunks), _ptr(rows), _ptr(chunk_bytes), _ptr(data)
+        b.n_series = int(n_series)
+        g = ffi.gpr_text_grid()
+        g.struct_size = C.sizeof(ffi.gpr_text_grid)
+        g.flags = (ffi.GPR_TEXT_FILL if fill and not resident else 0) | (ffi.GPR_TEXT_RESIDENT if resident else 0)
+        g.t_end, g.step = int(t_end), int(step)
+        g.window_seconds = int(T) * int(step) if window_seconds is None else int(window_seconds)
+        g.n_samples, g.n_rows = int(T), int(n_rows)
+        g.power_threshold = 0.0 if power_threshold is None else float(power_threshold)
+        st = ffi.gpr_sample_stats()
+        self._check(self._lib.gpr_chunks_scatter(self._h, C.byref(b), C.byref(g), plane, C.byref(st)))
+        return {"n_in": st.n_in, "n_oow": st.n_oow, "n_tiny": st.n_tiny}
+
     def resident_head(self) -> int:
         h = C.c_uint32()
         self._check(self._lib.gpr_resident_head(self._h, C.byref(h)))

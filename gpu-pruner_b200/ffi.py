@@ -93,6 +93,14 @@ class gpr_sample_stats(C.Structure):
     _fields_ = [("n_in", C.c_uint64), ("n_oow", C.c_uint64), ("n_tiny", C.c_uint64)]
 
 
+class gpr_chunk_batch(C.Structure):
+    _fields_ = [
+        ("struct_size", C.c_uint32), ("mem_kind", C.c_int32),
+        ("series_chunks", C.c_void_p), ("rows", C.c_void_p), ("chunk_bytes", C.c_void_p), ("data", C.c_void_p),
+        ("n_series", C.c_uint32), ("reserved", C.c_uint32),
+    ]
+
+
 GPR_SPAN_SHARED, GPR_SPAN_HARD = 1, 2
 GPR_TEXT_FILL, GPR_TEXT_RESIDENT = 1, 2
 
@@ -141,6 +149,8 @@ PROTOTYPES = {
     "gpr_text_planes": (C.c_int, [_P, C.POINTER(_P), C.POINTER(_P)]),
     "gpr_samples_scatter": (C.c_int, [_P, C.POINTER(gpr_sample_batch), C.POINTER(gpr_text_grid), C.c_int32,
                                       C.POINTER(gpr_sample_stats)]),
+    "gpr_chunks_scatter": (C.c_int, [_P, C.POINTER(gpr_chunk_batch), C.POINTER(gpr_text_grid), C.c_int32,
+                                     C.POINTER(gpr_sample_stats)]),
     "gpr_synth_fill": (C.c_int, [_P, C.c_uint64, C.c_int32, _P, C.c_uint64, C.c_uint32,
                                  C.c_uint32, C.c_uint32, C.c_uint64]),
     "gpr_synth_eligible": (C.c_int, [_P, C.c_uint64, _P, C.c_uint64, C.c_uint32]),

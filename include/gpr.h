@@ -495,6 +495,44 @@ typedef struct gpr_sample_stats gpr_sample_stats;
 GPR_API int gpr_samples_scatter(gpr_ctx *ctx, const gpr_sample_batch *batch, const gpr_text_grid *grid,
                                 int32_t plane, gpr_sample_stats *stats);
 
+/* ---- Prometheus XOR chunks into the same planes ------------------------------------------------------
+ * For a caller that reads series as stored chunks (Prometheus remote read with the STREAMED_XOR_CHUNKS
+ * response type, or a Thanos StoreAPI Series call): the `data` field of every XOR chunk, back to back in
+ * one buffer, decoded and merged on the GPU.  Framing, CRCs and label maps stay with the caller.
+ *
+ * CSR over chunks: series s owns chunks [series_chunks[s], series_chunks[s+1]) and feeds row rows[s];
+ * chunk c is data[chunk_bytes[c], chunk_bytes[c+1]), in Prometheus' XOR encoding (tsdb/chunkenc/xor.go:
+ * a big-endian u16 sample count, then the bit stream).  Chunks may overlap in time and come in any
+ * order.  Histogram chunks are not accepted.                                                         */
+struct gpr_chunk_batch {
+  uint32_t struct_size;           /* sizeof(gpr_chunk_batch)                                             */
+  int32_t mem_kind;               /* GPR_MEM_*: applies to every array below                             */
+  const uint64_t *series_chunks;  /* n_series + 1: series s owns chunks [series_chunks[s], series_chunks[s+1]) */
+  const uint32_t *rows;           /* n_series, each < grid.n_rows                                        */
+  const uint64_t *chunk_bytes;    /* n_chunks + 1: chunk c is data[chunk_bytes[c], chunk_bytes[c+1])     */
+  const uint8_t *data;            /* the XOR chunks' `data` fields, back to back, any alignment          */
+  uint32_t n_series;
+  uint32_t reserved;
+};
+typedef struct gpr_chunk_batch gpr_chunk_batch;
+
+/* Same destination, grid, flags and stats as gpr_samples_scatter: every decoded sample lands in the cell,
+ * with the f32 bits, that gpr_samples_scatter gives the same (ts_ms, value), and so gpr_text_parse.  NaN
+ * samples are dropped, Prometheus' staleness marker (0x7ff0000000000002) among them.  stats->n_in counts
+ * the decoded samples; a chunk's samples outside the window are counted in n_oow (chunks come whole, so a
+ * daemon slice has many).  The batch is checked before anything is written: a bad struct_size, offsets
+ * that do not start at 0 or decrease (series_chunks or chunk_bytes), a row >= grid.n_rows, a chunk
+ * shorter than its 2-byte header, a chunk whose decode would read past its own bytes (or whose varint
+ * overflows 64 bits), a value that reuses the XOR window before one was set, or (host batches) a chunk
+ * over 32 MB returns GPR_E_INVALID, naming the first bad chunk, with the destination untouched.  The
+ * index arrays of a host batch are checked on the host; chunk data, and every array of a device batch,
+ * by a check kernel whose verdict is read back before the merge.  Device arrays are read in place; host chunk data goes up in pieces cut at chunk
+ * boundaries through the staging of gpr_samples_scatter (a batch larger than two pieces, 64 MB, crosses
+ * PCIe twice: once to be checked, once to be merged).  stats may be NULL.  Blocking; results enqueued
+ * before the call stay pending.                                                                       */
+GPR_API int gpr_chunks_scatter(gpr_ctx *ctx, const gpr_chunk_batch *batch, const gpr_text_grid *grid,
+                               int32_t plane, gpr_sample_stats *stats);
+
 #ifdef __cplusplus
 }
 #endif
