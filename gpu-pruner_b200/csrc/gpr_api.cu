@@ -132,6 +132,11 @@ struct Buf {
     }
     return alloc(need + need / 4 + 64);
   }
+  // trade what is held with o (a buffer built beside this one takes its place)
+  void swap(Buf& o) {
+    std::swap(p, o.p);
+    std::swap(cap, o.cap);
+  }
 };
 template <typename T>
 using PinnedBuf = Buf<T, true>;
@@ -228,6 +233,11 @@ struct gpr_ctx {
   // is refused until gpr_resident_reindex has rebuilt it
   bool idx_stale = false;
   Buf<float> d_cols;
+  // gpr_resident_remap builds the new ring here, beside the old one, and the two change places once it is complete:
+  // [util, power, util index, power index]
+  Buf<float> d_res_next[4];
+  Buf<uint32_t> d_remap_map;            // a host map, uploaded
+  Buf<unsigned int> d_remap_check;      // a device map's check: [first bad new row | seen bitmap | dup bitmap]
 
   // device-side ingest of response text (gpr_text_scan / gpr_text_parse)
   Buf<uint8_t> d_text[3];
@@ -1380,6 +1390,98 @@ int gpr_append(gpr_ctx* ctx, const float* util_cols, const float* power_cols, ui
   }
   ctx->res_head = sp.next_head;
   CU(cudaStreamSynchronize(ctx->stream));
+  return GPR_OK;
+  GPR_CATCH(ctx)
+}
+
+// The first new row of a device map that gpr::remap_first_bad would name (n_new if none), by k_remap_check's two
+// passes; the old row it names goes to *src.
+static int remap_check_device(gpr_ctx* ctx, const uint32_t* src_rows, uint32_t n_new, uint32_t n_old, uint32_t* first,
+                              uint32_t* src) {
+  const size_t words = ((size_t)n_old + 31) / 32;
+  CU(ctx->d_remap_check.grow(ctx->stream, 1 + 2 * words));
+  unsigned int* d = ctx->d_remap_check;
+  CU(cudaMemsetAsync(d + 1, 0, 2 * words * sizeof(unsigned int), ctx->stream));
+  CU(cudaMemcpyAsync(d, &n_new, sizeof n_new, cudaMemcpyHostToDevice, ctx->stream));
+  const uint32_t blocks = std::max(1u, std::min((n_new + 255u) / 256u, (uint32_t)ctx->sm_count * 8u));
+  for (int pass = 0; pass < 2; ++pass) {
+    gpr::k_remap_check<<<blocks, 256, 0, ctx->stream>>>(src_rows, n_new, n_old, d + 1, d + 1 + words, d, pass);
+    ctx->launches++;
+    CU(cudaGetLastError());
+  }
+  CU(cudaMemcpyAsync(first, d, sizeof *first, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  if (*first < n_new) {
+    CU(cudaMemcpyAsync(src, src_rows + *first, sizeof *src, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
+  return GPR_OK;
+}
+
+// The new ring in d_res_next, gathered from the old one on the context's stream after whatever is enqueued there (the
+// decisions still pending read the old ring), and waited for.
+static int remap_build(gpr_ctx* ctx, const uint32_t* map, uint32_t n_rows) {
+  Buf<float>* cur[4] = {&ctx->d_res_util, &ctx->d_res_power, &ctx->d_idx_util, &ctx->d_idx_power};
+  const uint32_t len[4] = {ctx->res_T, ctx->res_T, ctx->idx_ld, ctx->idx_ld};
+  const uint32_t grid = gpr::ring_grid(n_rows, ctx->sm_count);
+  for (int k = 0; k < 4; ++k) {
+    if (!*cur[k]) continue;
+    CU(ctx->d_res_next[k].alloc((size_t)n_rows * len[k]));
+    gpr::k_remap_rows<<<grid, gpr::kRingThreads, 0, ctx->stream>>>(reinterpret_cast<uint32_t*>(ctx->d_res_next[k].p),
+                                                                  reinterpret_cast<const uint32_t*>(cur[k]->p), map,
+                                                                  n_rows, len[k]);
+    ctx->launches++;
+    CU(cudaGetLastError());
+  }
+  CU(cudaStreamSynchronize(ctx->stream));
+  return GPR_OK;
+}
+
+int gpr_resident_remap(gpr_ctx* ctx, uint32_t n_pods, uint32_t n_gpus, const uint32_t* src_rows, int32_t mem_kind) {
+  if (!ctx) return GPR_E_INVALID;
+  GPR_TRY
+  NvtxRange nvtx_range("gpr_resident_remap");
+  if (!ctx->d_res_util) return fail(ctx, GPR_E_STATE, "no resident window (gpr_resident_init)");
+  if (n_pods == 0 || n_gpus == 0) return fail(ctx, GPR_E_INVALID, "empty resident window");
+  if ((uint64_t)n_pods * n_gpus > 0x7fffffffull) return fail(ctx, GPR_E_INVALID, "too many series");
+  if (!src_rows) return fail(ctx, GPR_E_INVALID, "src_rows is NULL");
+  if (mem_kind != GPR_MEM_HOST && mem_kind != GPR_MEM_DEVICE) return fail(ctx, GPR_E_INVALID, "bad mem_kind %d", mem_kind);
+  CU(cudaSetDevice(ctx->device));
+  ctx->last_was_reduce = false;
+  const uint32_t n_new = n_pods * n_gpus, n_old = ctx->res_P * ctx->res_G;
+  // ---- the map is checked before the new ring is allocated or anything of the ring is written
+  uint32_t first = n_new, src = 0;
+  if (mem_kind == GPR_MEM_HOST) {
+    first = (uint32_t)gpr::remap_first_bad(src_rows, n_new, n_old);
+    if (first < n_new) src = src_rows[first];
+  } else {
+    const int rc = remap_check_device(ctx, src_rows, n_new, n_old, &first, &src);
+    if (rc != GPR_OK) return rc;
+  }
+  if (first < n_new && src >= n_old)
+    return fail(ctx, GPR_E_INVALID, "src_rows[%u] = %u: the resident window has %u rows (%u x %u)", first, src, n_old,
+                ctx->res_P, ctx->res_G);
+  if (first < n_new)
+    return fail(ctx, GPR_E_INVALID, "src_rows[%u] = %u: old row %u is the source of more than one new row", first, src,
+                src);
+  // ---- the new ring beside the old one; they change places only once it is complete
+  const uint32_t* map = src_rows;
+  if (mem_kind == GPR_MEM_HOST) {
+    CU(ctx->d_remap_map.grow(ctx->stream, n_new));
+    CU(cudaMemcpyAsync(ctx->d_remap_map, src_rows, (size_t)n_new * sizeof(uint32_t), cudaMemcpyHostToDevice,
+                       ctx->stream));
+    map = ctx->d_remap_map;
+  }
+  const int rc = remap_build(ctx, map, n_new);
+  if (rc != GPR_OK) {
+    (void)cudaStreamSynchronize(ctx->stream);  // a gather may still be writing a new buffer
+    for (Buf<float>& b : ctx->d_res_next) (void)b.release();
+    return rc;
+  }
+  Buf<float>* cur[4] = {&ctx->d_res_util, &ctx->d_res_power, &ctx->d_idx_util, &ctx->d_idx_power};
+  for (int k = 0; k < 4; ++k) cur[k]->swap(ctx->d_res_next[k]);
+  ctx->res_P = n_pods, ctx->res_G = n_gpus;
+  for (Buf<float>& b : ctx->d_res_next) CU(b.release());  // the old ring
   return GPR_OK;
   GPR_CATCH(ctx)
 }

@@ -4,13 +4,15 @@
 // The kernels here are plain CUDA C++ without inline PTX, and the host-side arithmetic of gpr_append /
 // gpr_resident_advance (which source columns survive, where they land, what each plane gets, the grid, the index
 // row length) is plain functions.  gpr_api.cu launches what these return; tests/cpp/ring_emul.cpp runs the same
-// source on the CPU against a numpy model of the ring.
+// source on the CPU against a numpy model of the ring.  gpr_resident_remap's row gather and map check are here too
+// (tests/cpp/remap_emul.cpp).
 #pragma once
 
 #include <stddef.h>
 #include <stdint.h>
 
 #include <algorithm>
+#include <vector>
 
 #include "gpr_kernels.cuh"
 
@@ -140,6 +142,75 @@ __global__ void __launch_bounds__(kRingThreads) k_reindex(const float* __restric
       const float m = block_max_warp(plane + (size_t)r * T, T, b, lane);
       if (lane == 0) idx[(size_t)r * idx_ld + b] = m;
     }
+}
+
+// ---- gpr_resident_remap: the ring's rows moved to a new [P][G] shape, out of place
+constexpr uint32_t kRowNone = 0xFFFFFFFFu;  // GPR_ROW_NONE: a new row without a source (no sample)
+
+// The first new row of a remap whose source is bad: an old row >= n_old that is not kRowNone, or an old row that is
+// also the source of another new row (every new row that shares it counts, the first of them included); n_new if the
+// map is good.  What k_remap_check computes on the GPU, for a host map.
+inline size_t remap_first_bad(const uint32_t* src_rows, size_t n_new, size_t n_old) {
+  std::vector<uint8_t> uses(n_old, 0);  // 0, 1, 2 = more than one
+  for (size_t i = 0; i < n_new; ++i)
+    if (src_rows[i] < n_old) uses[src_rows[i]] = (uint8_t)std::min(2, uses[src_rows[i]] + 1);
+  for (size_t i = 0; i < n_new; ++i) {
+    const uint32_t s = src_rows[i];
+    if (s == kRowNone) continue;
+    if (s >= n_old || uses[s] > 1) return i;
+  }
+  return n_new;
+}
+
+// k_remap_check's two passes over a device map (a grid-wide barrier between them: two launches).  `seen` and `dup`
+// are bitmaps of the n_old old rows, zeroed by the caller.  Pass 0 checks the range and marks every old row in `seen`,
+// and in `dup` if it was marked already; pass 1 names the new rows whose old row is in `dup`.  `first` (the caller
+// sets it to n_new) ends as remap_first_bad's answer.  Its minimum is an atomicMin written as a CAS loop, because
+// tests/cpp/cuda_shim.hpp, under which the CPU emulators compile this whole namespace, has atomicCAS and no atomicMin.
+__global__ void __launch_bounds__(256) k_remap_check(const uint32_t* __restrict__ src_rows, uint32_t n_new,
+                                                     uint32_t n_old, unsigned int* seen, unsigned int* dup,
+                                                     unsigned int* first, int pass) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_new; i += gridDim.x * blockDim.x) {
+    const uint32_t s = src_rows[i];
+    if (s == kRowNone) continue;
+    const unsigned int bit = 1u << (s % 32);
+    bool bad;
+    if (pass == 0) {
+      bad = s >= n_old;
+      if (!bad && (atomicOr(seen + s / 32, bit) & bit)) atomicOr(dup + s / 32, bit);
+    } else {
+      bad = s < n_old && (dup[s / 32] & bit);
+    }
+    if (!bad) continue;
+    unsigned int old = atomicOr(first, 0u);  // an atomic read
+    while (i < old) {
+      const unsigned int seen_first = atomicCAS(first, old, i);
+      if (seen_first == old) break;
+      old = seen_first;
+    }
+  }
+}
+
+// One new row of length `len` per CTA and round (grid: ring_grid): new row r is old row src_rows[r], or "no sample"
+// for kRowNone.  The same gather moves the planes (len = T) and their index (len = idx_ld, padding included, so it
+// stays NaN).  16-byte accesses when every row starts on a 16-byte boundary (len % 4 == 0), 4-byte ones otherwise.
+__global__ void __launch_bounds__(kRingThreads) k_remap_rows(uint32_t* __restrict__ dst,
+                                                             const uint32_t* __restrict__ src,
+                                                             const uint32_t* __restrict__ src_rows, uint32_t n_rows,
+                                                             uint32_t len) {
+  for (uint32_t r = blockIdx.x; r < n_rows; r += gridDim.x) {
+    const uint32_t s = src_rows[r];
+    uint32_t* out = dst + (size_t)r * len;
+    const uint32_t* in = s == kRowNone ? nullptr : src + (size_t)s * len;
+    if (len % 4u == 0) {
+      uint4* out4 = reinterpret_cast<uint4*>(out);
+      const uint4* in4 = reinterpret_cast<const uint4*>(in);
+      const uint4 none = make_uint4(kNoSampleBits, kNoSampleBits, kNoSampleBits, kNoSampleBits);
+      for (uint32_t j = threadIdx.x; j < len / 4u; j += blockDim.x) out4[j] = in ? in4[j] : none;
+    } else {
+      for (uint32_t j = threadIdx.x; j < len; j += blockDim.x) out[j] = in ? in[j] : kNoSampleBits;
+    }
+  }
 }
 
 }  // namespace gpr

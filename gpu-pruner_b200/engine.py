@@ -515,6 +515,27 @@ class IdleEngine:
         """open the next ``n_new`` buckets of the resident ring without data (all rows: no sample)"""
         self._check(self._lib.gpr_resident_advance(self._h, int(n_new)))
 
+    def resident_remap(self, P: int, G: int, src_rows):
+        """Give the resident ring the shape ``[P][G][T]`` without losing its history: new row ``i`` holds old row
+        ``src_rows[i]`` (uint32, ``P * G`` entries), or no sample for ``ffi.GPR_ROW_NONE``.  ``src_rows`` is a
+        numpy array (host) or a contiguous int32 / uint32 CUDA tensor on the engine's device (read in place; as
+        int32, ``GPR_ROW_NONE`` is -1)."""
+        if hasattr(src_rows, "is_cuda") and src_rows.is_cuda:
+            import torch
+            if src_rows.dtype not in (torch.int32, torch.uint32):
+                raise ValueError(f"src_rows must be an int32 or uint32 tensor, not {src_rows.dtype}")
+            if src_rows.device.index != self.device:
+                raise ValueError(f"src_rows is on {src_rows.device}, the engine on cuda:{self.device}")
+            if not src_rows.is_contiguous() or src_rows.numel() != P * G:
+                raise ValueError(f"src_rows must be a contiguous tensor of P * G = {P * G} entries")
+            self._check(self._lib.gpr_resident_remap(self._h, int(P), int(G), src_rows.data_ptr(),
+                                                     ffi.GPR_MEM_DEVICE))
+            return
+        rows = np.ascontiguousarray(src_rows, dtype=np.uint32).ravel()
+        if rows.size != P * G:
+            raise ValueError(f"src_rows has {rows.size} entries, not P * G = {P * G}")
+        self._check(self._lib.gpr_resident_remap(self._h, int(P), int(G), rows.ctypes.data, ffi.GPR_MEM_HOST))
+
     def text_planes(self):
         u, w = C.c_void_p(), C.c_void_p()
         self._check(self._lib.gpr_text_planes(self._h, C.byref(u), C.byref(w)))

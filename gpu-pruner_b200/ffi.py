@@ -103,6 +103,7 @@ class gpr_chunk_batch(C.Structure):
 
 GPR_SPAN_SHARED, GPR_SPAN_HARD = 1, 2
 GPR_TEXT_FILL, GPR_TEXT_RESIDENT = 1, 2
+GPR_ROW_NONE = 0xFFFFFFFF
 
 _P = C.c_void_p
 # name -> (restype, argtypes); must list every symbol include/gpr.h declares
@@ -122,6 +123,7 @@ PROTOTYPES = {
     "gpr_resident_head": (C.c_int, [_P, C.POINTER(C.c_uint32)]),
     "gpr_decide_resident": (C.c_int, [_P, C.POINTER(gpr_window), C.POINTER(gpr_result)]),
     "gpr_resident_planes": (C.c_int, [_P, C.POINTER(_P), C.POINTER(_P), C.POINTER(C.c_uint64)]),
+    "gpr_resident_remap": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P, C.c_int32]),
     "gpr_comm_unique_id": (C.c_int, [_P]),
     "gpr_comm_init": (C.c_int, [_P, _P, C.c_int, C.c_int]),
     "gpr_comm_destroy": (C.c_int, [_P]),

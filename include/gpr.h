@@ -277,6 +277,24 @@ GPR_API int gpr_decide_resident(gpr_ctx *ctx, const gpr_window *win, gpr_result 
 GPR_API int gpr_resident_planes(gpr_ctx *ctx, float **util, float **power, uint64_t *row_stride);
 /* ring position the next appended bucket goes to; the newest bucket is at (head + n_samples - 1) % n_samples  */
 GPR_API int gpr_resident_head(gpr_ctx *ctx, uint32_t *head);
+/* Give the ring a new shape [n_pods][n_gpus][n_samples] without losing its history: new row i
+ * (= pod * n_gpus + slot) holds old row src_rows[i] with every sample at its ring position, or no
+ * sample for GPR_ROW_NONE.  So pods can join beyond the head-room, a pod can gain series slots, and
+ * departed pods can be dropped without a query of the full window: the ring equals the one a rebuild
+ * from the full range would give if new row i were fed by the series that fed old row src_rows[i].
+ * n_samples, the head, the power plane and the GPR_F_BLOCK_INDEX index stay; index rows move with
+ * their rows (a stale index stays stale).  src_rows holds n_pods * n_gpus entries in host or device
+ * memory (mem_kind); it is checked before the new ring is allocated or the old one written (a
+ * device map's check uses context scratch of 2 bits per old row): an entry >= the old
+ * n_pods * n_gpus that is not GPR_ROW_NONE, or an old row named twice, is GPR_E_INVALID, and the
+ * message names the first new row whose entry is out of range or shared with another new row; no
+ * resident window is GPR_E_STATE.  On any error (GPR_E_NOMEM included) the ring, its index and its
+ * head are as they were.  Out of place: the new ring is built beside the old
+ * one, so the peak is the old ring plus the new one in HBM.  Decisions enqueued before the call read
+ * the old ring and retire at the next gpr_sync; pointers from gpr_resident_planes are stale after it.  */
+#define GPR_ROW_NONE 0xFFFFFFFFu
+GPR_API int gpr_resident_remap(gpr_ctx *ctx, uint32_t n_pods, uint32_t n_gpus, const uint32_t *src_rows,
+                               int32_t mem_kind);
 
 /* ---- multi-GPU: one process per GPU, pods sharded by rank, one allgather of the bitmap - */
 #define GPR_UNIQUE_ID_BYTES 128
