@@ -33,6 +33,7 @@
 #include "gpr_text_kernels.cuh"
 #include "gpr_samples.cuh"
 #include "gpr_chunks.cuh"
+#include "gpr_chunks_encode.cuh"
 
 namespace {
 
@@ -280,6 +281,12 @@ struct gpr_ctx {
   // XOR chunks (gpr_chunks_scatter) share that staging, and d_soffsets / d_srows for a host batch's series_chunks
   // and rows
   Buf<uint64_t> d_cbytes;              // a host batch's chunk_bytes, uploaded whole (8 B per chunk)
+  // the resident ring exported as XOR chunks (gpr_resident_export, gpr_chunks_encode.cuh)
+  Buf<uint32_t> d_xsizes;              // [rows][ceil(T / per_chunk)]: the bytes of each chunk
+  Buf<uint64_t> d_xrows;               // [2][rows + 1]: chunks and bytes per row, then their exclusive scans
+  Buf<uint32_t> d_xseries;             // [rows + 1]: the series index of each row
+  Buf<unsigned long long> d_xtotals;   // [4]: chunks, bytes, series, samples
+  Buf<unsigned char> d_xout;           // host outputs, encoded here first: [series_chunks | chunk_bytes | rows | data]
 
   // multi-GPU
   ncclComm_t comm = nullptr;
@@ -2323,6 +2330,94 @@ int gpr_chunks_scatter(gpr_ctx* ctx, const gpr_chunk_batch* batch, const gpr_tex
   CU(cudaMemcpyAsync(counts, ctx->d_sstats, sizeof counts, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   if (stats) stats->n_in = back[1], stats->n_oow = counts[0], stats->n_tiny = counts[1];
+  return GPR_OK;
+  GPR_CATCH(ctx)
+}
+
+// ---- the resident ring as XOR chunks (gpr_chunks_encode.cuh) --------------------------------------------------
+static_assert(sizeof(gpr_chunk_export) == 96, "gpr_chunk_export");
+
+static uint32_t export_grid(gpr_ctx* ctx, uint32_t rows) {
+  namespace gc = gpr::chunks;
+  return (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)rows + gc::kEncWarps - 1) / gc::kEncWarps,
+                                                            (uint64_t)ctx->sm_count * 16));
+}
+
+int gpr_resident_export(gpr_ctx* ctx, const gpr_text_grid* grid, int32_t plane, uint32_t max_per_chunk,
+                        gpr_chunk_export* out) {
+  if (!ctx) return GPR_E_INVALID;
+  GPR_TRY
+  NvtxRange nvtx_range("gpr_resident_export");
+  namespace gc = gpr::chunks;
+  if (!out || out->struct_size != sizeof(gpr_chunk_export))
+    return fail(ctx, GPR_E_INVALID, "out is NULL / struct_size mismatch");
+  out->n_series = out->n_chunks = out->n_bytes = out->n_samples = 0;
+  if (!grid || grid->struct_size != sizeof(gpr_text_grid)) return fail(ctx, GPR_E_INVALID, "grid is NULL / struct_size mismatch");
+  if (plane < 0 || plane > 1) return fail(ctx, GPR_E_INVALID, "bad plane %d", plane);
+  if (out->mem_kind != GPR_MEM_HOST && out->mem_kind != GPR_MEM_DEVICE)
+    return fail(ctx, GPR_E_INVALID, "bad mem_kind %d", out->mem_kind);
+  if (max_per_chunk < 1 || max_per_chunk > 65535)
+    return fail(ctx, GPR_E_INVALID, "max_per_chunk %u is outside 1..65535 (a chunk counts its samples in a u16)",
+                max_per_chunk);
+  if (!out->series_chunks || (out->cap_series && !out->rows) || !out->chunk_bytes || (out->cap_bytes && !out->data))
+    return fail(ctx, GPR_E_INVALID, "series_chunks / rows / chunk_bytes / data is NULL");
+  if (!ctx->d_res_util) return fail(ctx, GPR_E_STATE, "no resident window (gpr_resident_init)");
+  if (plane == 1 && !ctx->d_res_power) return fail(ctx, GPR_E_STATE, "the resident window has no power plane");
+  int rc;
+  if ((rc = check_grid(ctx, grid)) != GPR_OK) return rc;
+  if (grid->n_samples != ctx->res_T)
+    return fail(ctx, GPR_E_INVALID, "grid.n_samples %u is not the resident window's %u", grid->n_samples, ctx->res_T);
+  CU(cudaSetDevice(ctx->device));
+  ctx->last_was_reduce = false;
+  const uint32_t rows = ctx->res_P * ctx->res_G, T = ctx->res_T;
+  gc::ExportArgs a;
+  memset(&a, 0, sizeof a);
+  a.plane = reinterpret_cast<const uint32_t*>(plane == 0 ? ctx->d_res_util.p : ctx->d_res_power.p);
+  a.rows = rows, a.T = T, a.head = ctx->res_head, a.per_chunk = max_per_chunk;
+  a.t_end_ms = grid->t_end * 1000, a.step_ms = grid->step * 1000;
+  a.max_chunks = (T + max_per_chunk - 1) / max_per_chunk;
+  // ---- sizes, and their scan
+  CU(ctx->d_xsizes.grow(ctx->stream, (size_t)rows * a.max_chunks));
+  CU(ctx->d_xrows.grow(ctx->stream, 2 * ((size_t)rows + 1)));
+  CU(ctx->d_xseries.grow(ctx->stream, (size_t)rows + 1));
+  CU(ctx->d_xtotals.alloc_once(4));
+  a.sizes = ctx->d_xsizes, a.row_chunks = ctx->d_xrows, a.row_bytes = ctx->d_xrows + rows + 1;
+  a.row_series = ctx->d_xseries, a.totals = ctx->d_xtotals;
+  CU(cudaMemsetAsync(a.totals, 0, 4 * sizeof(unsigned long long), ctx->stream));
+  const uint32_t blocks = export_grid(ctx, rows);
+  gc::k_export_size<<<blocks, gc::kEncThreads, 0, ctx->stream>>>(a);
+  gc::k_export_scan<<<1, gc::kScanThreads, gc::kScanSmem, ctx->stream>>>(a);
+  ctx->launches += 2;
+  CU(cudaGetLastError());
+  unsigned long long tot[4];
+  CU(cudaMemcpyAsync(tot, a.totals, sizeof tot, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  out->n_chunks = tot[0], out->n_bytes = tot[1], out->n_series = tot[2], out->n_samples = tot[3];
+  if (out->n_series > out->cap_series || out->n_chunks > out->cap_chunks || out->n_bytes > out->cap_bytes)
+    return fail(ctx, GPR_E_CAPACITY, "%llu series, %llu chunks, %llu bytes; room for %llu, %llu, %llu: call again with "
+                "larger capacities", tot[2], tot[0], tot[1], (unsigned long long)out->cap_series,
+                (unsigned long long)out->cap_chunks, (unsigned long long)out->cap_bytes);
+  // ---- the outputs: in place on the device, or in context scratch copied out once per array
+  const size_t b_sc = (tot[2] + 1) * 8, b_cb = (tot[0] + 1) * 8, b_rows = tot[2] * 4, b_data = tot[1];
+  const bool host = out->mem_kind == GPR_MEM_HOST;
+  if (host) {
+    CU(ctx->d_xout.grow(ctx->stream, b_sc + b_cb + b_rows + b_data));
+    unsigned char* o = ctx->d_xout;
+    a.series_chunks = reinterpret_cast<uint64_t*>(o), a.chunk_bytes = reinterpret_cast<uint64_t*>(o + b_sc);
+    a.out_rows = reinterpret_cast<uint32_t*>(o + b_sc + b_cb), a.data = o + b_sc + b_cb + b_rows;
+  } else {
+    a.series_chunks = out->series_chunks, a.out_rows = out->rows, a.chunk_bytes = out->chunk_bytes, a.data = out->data;
+  }
+  gc::k_export_write<<<blocks, gc::kEncThreads, 0, ctx->stream>>>(a);
+  ctx->launches++;
+  CU(cudaGetLastError());
+  if (host) {
+    CU(cudaMemcpyAsync(out->series_chunks, a.series_chunks, b_sc, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(out->chunk_bytes, a.chunk_bytes, b_cb, cudaMemcpyDeviceToHost, ctx->stream));
+    if (b_rows) CU(cudaMemcpyAsync(out->rows, a.out_rows, b_rows, cudaMemcpyDeviceToHost, ctx->stream));
+    if (b_data) CU(cudaMemcpyAsync(out->data, a.data, b_data, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  CU(cudaStreamSynchronize(ctx->stream));
   return GPR_OK;
   GPR_CATCH(ctx)
 }

@@ -506,6 +506,40 @@ class IdleEngine:
         self._check(self._lib.gpr_chunks_scatter(self._h, C.byref(b), C.byref(g), plane, C.byref(st)))
         return {"n_in": st.n_in, "n_oow": st.n_oow, "n_tiny": st.n_tiny}
 
+    def resident_export(self, t_end: int, step: int, *, plane: int = 0, max_per_chunk: int = 120,
+                        window_seconds: Optional[int] = None, power_threshold: Optional[float] = 0.0) -> dict:
+        """Encode one plane of the resident ring (0 = util, 1 = power) as Prometheus XOR chunks on the GPU
+        (gpr_resident_export): every row with a sample is a series, its cells oldest first at
+        ``t_end - (T - 1 - j) * step`` seconds.  Returns numpy arrays ready for :meth:`chunks_scatter`
+        (``series_chunks``, ``rows``, ``chunk_bytes``, ``data``), the counts ``n_samples``, and the ``grid`` to
+        restore with: ``chunks_scatter(..., **out["grid"], resident=True)`` into a ring of the same T."""
+        T = int(self.resident_planes()[2])
+        g = ffi.gpr_text_grid()
+        g.struct_size = C.sizeof(ffi.gpr_text_grid)
+        g.t_end, g.step = int(t_end), int(step)
+        g.window_seconds = T * int(step) if window_seconds is None else int(window_seconds)
+        g.n_samples = T
+        g.power_threshold = 0.0 if power_threshold is None else float(power_threshold)
+        o = ffi.gpr_chunk_export()
+        o.struct_size = C.sizeof(ffi.gpr_chunk_export)
+        o.mem_kind = ffi.GPR_MEM_HOST
+        arrays = None
+        for _ in range(2):   # the sizes, then the chunks
+            if arrays is None:
+                arrays = (np.zeros(1, np.uint64), np.zeros(0, np.uint32), np.zeros(1, np.uint64), np.zeros(0, np.uint8))
+            o.series_chunks, o.rows, o.chunk_bytes, o.data = (_ptr(a) if a.size else None for a in arrays)
+            o.cap_series, o.cap_chunks, o.cap_bytes = arrays[1].size, arrays[2].size - 1, arrays[3].size
+            rc = self._lib.gpr_resident_export(self._h, C.byref(g), int(plane), int(max_per_chunk), C.byref(o))
+            if rc != ffi.GPR_E_CAPACITY:
+                break
+            arrays = (np.zeros(o.n_series + 1, np.uint64), np.zeros(o.n_series, np.uint32),
+                      np.zeros(o.n_chunks + 1, np.uint64), np.zeros(o.n_bytes, np.uint8))
+        self._check(rc)
+        return {"series_chunks": arrays[0], "rows": arrays[1], "chunk_bytes": arrays[2], "data": arrays[3],
+                "n_samples": int(o.n_samples),
+                "grid": {"t_end": int(t_end), "step": int(step), "T": T, "window_seconds": int(g.window_seconds),
+                         "plane": int(plane), "power_threshold": g.power_threshold}}
+
     def resident_head(self) -> int:
         h = C.c_uint32()
         self._check(self._lib.gpr_resident_head(self._h, C.byref(h)))

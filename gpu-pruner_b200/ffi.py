@@ -101,6 +101,15 @@ class gpr_chunk_batch(C.Structure):
     ]
 
 
+class gpr_chunk_export(C.Structure):
+    _fields_ = [
+        ("struct_size", C.c_uint32), ("mem_kind", C.c_int32),
+        ("series_chunks", C.c_void_p), ("rows", C.c_void_p), ("chunk_bytes", C.c_void_p), ("data", C.c_void_p),
+        ("cap_series", C.c_uint64), ("cap_chunks", C.c_uint64), ("cap_bytes", C.c_uint64),
+        ("n_series", C.c_uint64), ("n_chunks", C.c_uint64), ("n_bytes", C.c_uint64), ("n_samples", C.c_uint64),
+    ]
+
+
 GPR_SPAN_SHARED, GPR_SPAN_HARD = 1, 2
 GPR_TEXT_FILL, GPR_TEXT_RESIDENT = 1, 2
 GPR_ROW_NONE = 0xFFFFFFFF
@@ -153,6 +162,8 @@ PROTOTYPES = {
                                       C.POINTER(gpr_sample_stats)]),
     "gpr_chunks_scatter": (C.c_int, [_P, C.POINTER(gpr_chunk_batch), C.POINTER(gpr_text_grid), C.c_int32,
                                      C.POINTER(gpr_sample_stats)]),
+    "gpr_resident_export": (C.c_int, [_P, C.POINTER(gpr_text_grid), C.c_int32, C.c_uint32,
+                                      C.POINTER(gpr_chunk_export)]),
     "gpr_synth_fill": (C.c_int, [_P, C.c_uint64, C.c_int32, _P, C.c_uint64, C.c_uint32,
                                  C.c_uint32, C.c_uint32, C.c_uint64]),
     "gpr_synth_eligible": (C.c_int, [_P, C.c_uint64, _P, C.c_uint64, C.c_uint32]),

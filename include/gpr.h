@@ -551,6 +551,53 @@ typedef struct gpr_chunk_batch gpr_chunk_batch;
 GPR_API int gpr_chunks_scatter(gpr_ctx *ctx, const gpr_chunk_batch *batch, const gpr_text_grid *grid,
                                int32_t plane, gpr_sample_stats *stats);
 
+/* ---- the resident ring as XOR chunks: a snapshot a restarted caller restores ---------------------------
+ * gpr_resident_export encodes one plane of the ring (0 = util, 1 = power) on the GPU as Prometheus XOR
+ * chunks, in the CSR form gpr_chunks_scatter takes.  Every ring row with a sample is one series; its
+ * samples are its cells oldest first, sample j (ring position (head + j) % n_samples) at
+ *   ts_ms = grid.t_end * 1000 - (n_samples - 1 - j) * grid.step * 1000,   value = (double)cell,
+ * NaN cells skipped, cut into chunks of at most max_per_chunk samples (Prometheus cuts at 120).  The bytes
+ * are those Prometheus' appender writes for the same samples.
+ *
+ * Sizes follow the two calls of gpr_text_scan: with a capacity too small (n_series > cap_series,
+ * n_chunks > cap_chunks or n_bytes > cap_bytes) the call returns GPR_E_CAPACITY with the true counts and
+ * writes none of the five arrays; call again with room.  The counts are filled whenever the ring was
+ * encoded.  Errors: a bad struct_size, grid (as gpr_chunks_scatter checks it), grid.n_samples other than
+ * the ring's, mem_kind, a NULL series_chunks or chunk_bytes (or rows / data with room), or max_per_chunk
+ * outside 1..65535 is GPR_E_INVALID; no
+ * resident window, or plane 1 on a ring without a power plane, is GPR_E_STATE.  grid.n_rows and
+ * grid.flags are ignored; grid.window_seconds is for the restore.  Device outputs are written in
+ * place; host outputs (pinned or pageable) are encoded into context scratch and copied out, each array
+ * once.  Context scratch: 4 B per chunk the ring could hold (n_samples / max_per_chunk rounded up, per row)
+ * and 20 B per row, plus the outputs for host ones.  The ring, its head and its index are only read.
+ * Blocking; results enqueued before the call stay pending.
+ *
+ * Restore: gpr_resident_init with the same n_samples, then gpr_chunks_scatter(GPR_TEXT_RESIDENT) with the
+ * same grid and power_threshold (and `rows` mapped through the caller's pod table if the shape changed),
+ * then gpr_resident_reindex.  This gives a ring whose unrolled window equals the exported one bit for bit
+ * (every NaN reads back as the fill 0xFFFFFFFF) when every column is inside the grid's window:
+ * (n_samples - 1) * step < window_seconds, as with n_samples = ceil(window_seconds / step).  DESIGN.md §8h
+ * gives the argument.                                                                                   */
+struct gpr_chunk_export {
+  uint32_t struct_size;    /* sizeof(gpr_chunk_export)                                                  */
+  int32_t mem_kind;        /* GPR_MEM_*: where the four arrays below live                               */
+  uint64_t *series_chunks; /* cap_series + 1: series s owns chunks [series_chunks[s], series_chunks[s+1]) */
+  uint32_t *rows;          /* cap_series: the ring row of each exported series, ascending               */
+  uint64_t *chunk_bytes;   /* cap_chunks + 1: chunk c is data[chunk_bytes[c], chunk_bytes[c+1])          */
+  uint8_t *data;           /* cap_bytes: the chunks, back to back                                       */
+  uint64_t cap_series;
+  uint64_t cap_chunks;
+  uint64_t cap_bytes;
+  uint64_t n_series;       /* out: rows with at least one sample                                        */
+  uint64_t n_chunks;       /* out                                                                        */
+  uint64_t n_bytes;        /* out                                                                        */
+  uint64_t n_samples;      /* out: present cells                                                        */
+};
+typedef struct gpr_chunk_export gpr_chunk_export;
+
+GPR_API int gpr_resident_export(gpr_ctx *ctx, const gpr_text_grid *grid, int32_t plane,
+                                uint32_t max_per_chunk, gpr_chunk_export *out);
+
 #ifdef __cplusplus
 }
 #endif
