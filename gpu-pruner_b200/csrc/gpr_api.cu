@@ -23,6 +23,7 @@
 #include <mutex>
 #include <new>
 #include <thread>
+#include <utility>
 #include <vector>
 
 #include "gpr_kernels.cuh"
@@ -273,7 +274,7 @@ struct gpr_ctx {
   // two device buffers (and, for pageable memory, two pinned ones): piece k + 1 is copied while piece k is scattered.
   Buf<uint64_t> d_soffsets;            // a host batch's offsets and rows, uploaded whole (12 B per series)
   Buf<uint32_t> d_srows;
-  Buf<unsigned long long> d_sstats;    // [n_oow, n_tiny, check word of a device batch]
+  Buf<unsigned long long> d_sstats;    // [n_oow, n_tiny, check word, n_in, first bad chunk]
   Buf<unsigned char> d_sstage;         // [2][ts kHostPiece | values kHostPiece]
   PinnedBuf<unsigned char> h_sstage;   // the same, pinned
   Event ev_sup[2];                     // piece in buffer b uploaded
@@ -353,6 +354,18 @@ int env_int(const char* name, int dflt) {
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
+// Whether both host arrays are pinned (registered with CUDA); pageable ones go up through pinned staging.
+bool host_pinned(const void* a, const void* b) {
+  bool pinned = true;
+  for (const void* p : {a, b}) {
+    if (!p) continue;
+    cudaPointerAttributes at;
+    pinned = pinned && cudaPointerGetAttributes(&at, p) == cudaSuccess && at.type == cudaMemoryTypeHost;
+    (void)cudaGetLastError();  // an unregistered pointer may leave an error code behind
+  }
+  return pinned;
+}
+
 // smallest f32 >= thr, so that (m >= thr_f) in f32 equals ((double)m >= thr) for every f32 m
 float threshold_f32(double thr) { return gpr::text::threshold_up(thr); }
 
@@ -371,24 +384,37 @@ gpr::LaunchKnobs launch_knobs(const gpr_ctx* ctx) {
   return k;
 }
 
-// One launch helper for both variants; `pdl` adds the programmatic-stream-serialization
-// attribute so the kernel may begin while the previous reduce kernel on the stream drains.
+// The prologue of every entry point that enqueues work on the context's stream or waits for it.  Whatever the call
+// enqueues is not one of our folds, so the next decision's reduce must not start early behind it (programmatic
+// dependent launch is requested only while last_was_reduce holds, DESIGN.md §4).
+int enter(gpr_ctx* ctx) {
+  ctx->last_was_reduce = false;
+  CU(cudaSetDevice(ctx->device));
+  return GPR_OK;
+}
+
+// Every kernel on the context's stream is launched here, and counted (gpr_launch_count).  `pdl` adds the
+// programmatic-stream-serialization attribute so the kernel may begin while the previous reduce kernel on the stream
+// drains.
 template <typename Kernel, typename... Args>
-cudaError_t launch_ex(Kernel k, uint32_t grid, uint32_t block, size_t smem, cudaStream_t st, bool pdl,
-                      Args... args) {
+int launch(gpr_ctx* ctx, Kernel k, uint32_t grid, uint32_t block, size_t smem, bool pdl, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid), cfg.blockDim = dim3(block), cfg.dynamicSmemBytes = smem, cfg.stream = st;
+  cfg.gridDim = dim3(grid), cfg.blockDim = dim3(block), cfg.dynamicSmemBytes = smem, cfg.stream = ctx->stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, k, args...);
+  ctx->launches++;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, k, std::forward<Args>(args)...);
+  CU(cudaGetLastError());  // (a failed launch leaves its error here too: this clears it)
+  CU(e);
+  return GPR_OK;
 }
 
-template <int NW, bool kGroups>
-cudaError_t launch_tma(gpr_ctx* ctx, const gpr::ReduceParams& rp, const gpr::ReducePlan& plan, bool pdl) {
-  return launch_ex(gpr::k_reduce_tma<NW, kGroups>, plan.grid, plan.block, plan.smem, ctx->stream, pdl, rp, plan.L);
+// ceil(n / per_cta) CTAs, at most per_sm per SM and at least one
+uint32_t capped_grid(const gpr_ctx* ctx, uint64_t n, uint64_t per_cta, uint32_t per_sm) {
+  return (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n + per_cta - 1) / per_cta, (uint64_t)ctx->sm_count * per_sm));
 }
 
 // launch one reduce pass over the rows described by rp (kGroups: the instantiation for a group table)
@@ -401,24 +427,19 @@ int launch_reduce_as(gpr_ctx* ctx, gpr::ReduceParams& rp, bool tma_ok, bool pdl)
   const bool may_stop = !kGroups && rp.seg[0].smax == nullptr && rp.seg[1].smax == nullptr;
   const gpr::ReducePlan plan =
       gpr::plan_reduce(launch_knobs(ctx), rp.T, rp.total_rows, tma_ok, rp.util_u8 != 0, may_stop);
-  cudaError_t e;
-  if (plan.kernel == gpr::kReduceProbe) {
-    e = launch_ex(gpr::k_reduce_probe<gpr::kProbeWarps>, plan.grid, plan.block, plan.smem, ctx->stream, pdl, rp, plan.L);
-  } else if (plan.kernel == gpr::kReduceU8) {
-    e = launch_ex(gpr::k_reduce_u8<kLdgWarps, gpr::kU8Unroll, kGroups>, plan.grid, plan.block, 0, ctx->stream, pdl, rp);
-  } else if (plan.kernel == gpr::kReduceTma) {
+  if (plan.kernel == gpr::kReduceProbe)
+    return launch(ctx, gpr::k_reduce_probe<gpr::kProbeWarps>, plan.grid, plan.block, plan.smem, pdl, rp, plan.L);
+  if (plan.kernel == gpr::kReduceU8)
+    return launch(ctx, gpr::k_reduce_u8<kLdgWarps, gpr::kU8Unroll, kGroups>, plan.grid, plan.block, 0, pdl, rp);
+  if (plan.kernel == gpr::kReduceTma) {
     const int nw = ctx->tma_warps;
-    if (nw == 4) e = launch_tma<4, kGroups>(ctx, rp, plan, pdl);
-    else if (nw == 16) e = launch_tma<16, kGroups>(ctx, rp, plan, pdl);
-    else if (nw == 32) e = launch_tma<32, kGroups>(ctx, rp, plan, pdl);
-    else e = launch_tma<8, kGroups>(ctx, rp, plan, pdl);
-  } else {
-    e = launch_ex(gpr::k_reduce_ldg<kLdgWarps, kLdgUnroll, kGroups>, plan.grid, plan.block, 0, ctx->stream, pdl, rp);
+    const auto k = nw == 4    ? gpr::k_reduce_tma<4, kGroups>
+                   : nw == 16 ? gpr::k_reduce_tma<16, kGroups>
+                   : nw == 32 ? gpr::k_reduce_tma<32, kGroups>
+                              : gpr::k_reduce_tma<8, kGroups>;
+    return launch(ctx, k, plan.grid, plan.block, plan.smem, pdl, rp, plan.L);
   }
-  ctx->launches++;
-  CU(e);
-  CU(cudaGetLastError());
-  return GPR_OK;
+  return launch(ctx, gpr::k_reduce_ldg<kLdgWarps, kLdgUnroll, kGroups>, plan.grid, plan.block, 0, pdl, rp);
 }
 int launch_reduce(gpr_ctx* ctx, gpr::ReduceParams& rp, bool tma_ok, bool pdl) {
   return rp.grouped ? launch_reduce_as<true>(ctx, rp, tma_ok, pdl) : launch_reduce_as<false>(ctx, rp, tma_ok, pdl);
@@ -690,22 +711,16 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
   const uint32_t group_grid = gpr::group_grid(launch_knobs(ctx), P);
   auto launch_group_rows = [&]() -> int {
     CU(cudaMemsetAsync(ctx->d_gpods, 0, sizeof(uint32_t), ctx->stream));
-    CU(launch_ex(gpr::k_group_rows, group_grid, gpr::kGroupBlock, 0, ctx->stream, false, gq));
-    ctx->launches++;
-    return GPR_OK;
+    return launch(ctx, gpr::k_group_rows, group_grid, gpr::kGroupBlock, 0, false, gq);
   };
   auto launch_group_sum = [&]() -> int {
-    CU(launch_ex(gpr::k_group_sum, group_grid, gpr::kGroupBlock, 0, ctx->stream, false, gq));
-    ctx->launches++;
-    return GPR_OK;
+    return launch(ctx, gpr::k_group_sum, group_grid, gpr::kGroupBlock, 0, false, gq);
   };
   const bool fold_pdl = can_pdl && !grouped;
-  auto launch_fold = [&](bool pdl) -> cudaError_t {
-    if (fused)
-      return islots_dev ? launch_ex(gpr::k_fold<true, true>, fold_grid, fold_threads, 0, ctx->stream, pdl, fp)
-                        : launch_ex(gpr::k_fold<true, false>, fold_grid, fold_threads, 0, ctx->stream, pdl, fp);
-    return islots_dev ? launch_ex(gpr::k_fold<false, true>, fold_grid, fold_threads, 0, ctx->stream, pdl, fp)
-                      : launch_ex(gpr::k_fold<false, false>, fold_grid, fold_threads, 0, ctx->stream, pdl, fp);
+  auto launch_fold = [&](bool pdl) -> int {
+    const auto k = fused ? (islots_dev ? gpr::k_fold<true, true> : gpr::k_fold<true, false>)
+                         : (islots_dev ? gpr::k_fold<false, true> : gpr::k_fold<false, false>);
+    return launch(ctx, k, fold_grid, fold_threads, 0, pdl, fp);
   };
 
   if (!async) {
@@ -732,8 +747,7 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
       if (grouped && (rc = launch_group_rows()) != GPR_OK) return rc;
       if ((rc = launch_reduce(ctx, rp, tma_ok, pdl)) != GPR_OK) return rc;
       if (grouped && (rc = launch_group_sum()) != GPR_OK) return rc;
-      CU(launch_fold(fold_pdl));
-      ctx->launches++;
+      if ((rc = launch_fold(fold_pdl)) != GPR_OK) return rc;
       ctx->uses[sset]++;
       ctx->last_was_reduce = !grouped;
     }
@@ -779,8 +793,7 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
     }
     if (grouped && (rc = launch_group_sum()) != GPR_OK) return rc;
     if (P > 0) {
-      CU(launch_fold(false));
-      ctx->launches++;
+      if ((rc = launch_fold(false)) != GPR_OK) return rc;
       ctx->uses[sset]++;
     }
   }
@@ -972,7 +985,7 @@ void scan_producer(gpr_ctx* ctx, ScanPipe* sp, int k) {
     if (e != cudaSuccess) break;
     const uint64_t s0 = off / gpr::text::kScanBytes;
     const uint64_t s1 = (off + len + gpr::text::kScanBytes - 1) / gpr::text::kScanBytes;
-    const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((s1 - s0 + 255) / 256, (uint64_t)ctx->sm_count * 8));
+    const uint32_t grid = capped_grid(ctx, s1 - s0, 256, 8);
     k_text_scan_chunk<<<grid, 256, 0, st>>>(sp->dst, sp->n, s0, s1, ctx->d_mark_blocks, sp->unit, u0);
     k_publish_marks<<<(uint32_t)nu, 256, 0, st>>>(ctx->d_mark_blocks, ctx->h_mark_blocks, u0);
     e = cudaGetLastError();
@@ -1018,11 +1031,11 @@ int check_grid(gpr_ctx* ctx, const gpr_text_grid* grid) {
   return GPR_OK;
 }
 
-// Where gpr_text_parse and gpr_samples_scatter merge samples, and its time axis in milliseconds (the resolution of
-// Prometheus timestamps): the resident ring (GPR_TEXT_RESIDENT) or the context plane `plane`, grown to the grid
-// (a plane that has to grow must be filled).  Writes no cell: filling the plane (GPR_TEXT_FILL) and marking the
-// ring's index stale are the caller's.
-int text_destination(gpr_ctx* ctx, const gpr_text_grid* grid, int32_t plane, gpr::text::Grid* g, float** pl) {
+// Where gpr_text_parse, gpr_samples_scatter and gpr_chunks_scatter merge samples, and its time axis in milliseconds
+// (the resolution of Prometheus timestamps): the resident ring (GPR_TEXT_RESIDENT) or the context plane `plane`, grown
+// to the grid (a plane that has to grow must be filled).  The caller has checked everything else, so the merge is
+// certain once this succeeds: it fills the plane (GPR_TEXT_FILL) or marks the ring's index stale.
+int open_destination(gpr_ctx* ctx, const gpr_text_grid* grid, int32_t plane, gpr::text::Grid* g, float** pl) {
   const uint32_t n_samples = grid->n_samples, n_rows = grid->n_rows;
   memset(g, 0, sizeof *g);
   g->t_end = grid->t_end * 1000, g->t_lo = (grid->t_end - grid->window_seconds) * 1000;
@@ -1037,6 +1050,7 @@ int text_destination(gpr_ctx* ctx, const gpr_text_grid* grid, int32_t plane, gpr
     if (!*pl) return fail(ctx, GPR_E_STATE, "the resident window has no power plane");
     g->ld = ctx->res_T;
     g->col_end = (ctx->res_head + ctx->res_T - 1) % ctx->res_T;  // the newest bucket sits just before the head
+    if (ctx->d_idx_util) ctx->idx_stale = true;  // the merge does not touch the index (gpr_resident_reindex)
   } else {
     const size_t cells = (size_t)n_rows * n_samples;
     const size_t cap_before = ctx->d_tplane[plane].cap;
@@ -1045,18 +1059,8 @@ int text_destination(gpr_ctx* ctx, const gpr_text_grid* grid, int32_t plane, gpr
       return fail(ctx, GPR_E_STATE, "plane %d had to grow: the first parse of a window must pass GPR_TEXT_FILL", plane);
     *pl = ctx->d_tplane[plane];
     g->ld = n_samples, g->col_end = n_samples - 1;
-  }
-  return GPR_OK;
-}
-
-// the fill of a context plane (GPR_TEXT_FILL) and the stale mark of the ring's index, once the merge is certain
-int open_destination(gpr_ctx* ctx, const gpr_text_grid* grid, float* pl) {
-  if (grid->flags & GPR_TEXT_RESIDENT) {
-    if (ctx->d_idx_util) ctx->idx_stale = true;  // the merge does not touch the index (gpr_resident_reindex)
-  } else if (grid->flags & GPR_TEXT_FILL) {
     // 0xFFFFFFFF: a NaN, and -1 as an int — below every non-negative sample for the integer atomicMax merge
-    const size_t cells = (size_t)grid->n_rows * grid->n_samples;
-    if (cells) CU(cudaMemsetAsync(pl, 0xFF, cells * sizeof(float), ctx->stream));
+    if ((grid->flags & GPR_TEXT_FILL) && cells) CU(cudaMemsetAsync(*pl, 0xFF, cells * sizeof(float), ctx->stream));
   }
   return GPR_OK;
 }
@@ -1292,9 +1296,9 @@ int gpr_decide_resident(gpr_ctx* ctx, const gpr_window* win, gpr_result* res) {
 int gpr_resident_init(gpr_ctx* ctx, uint32_t P, uint32_t G, uint32_t T, uint32_t flags) {
   if (!ctx) return GPR_E_INVALID;
   GPR_TRY
+  if (const int rc = enter(ctx)) return rc;
   if (P == 0 || G == 0 || T == 0) return fail(ctx, GPR_E_INVALID, "empty resident window");
   if ((uint64_t)P * G > 0x7fffffffull) return fail(ctx, GPR_E_INVALID, "too many series");
-  CU(cudaSetDevice(ctx->device));
   CU(cudaStreamSynchronize(ctx->stream));
   for (Buf<float>* b : {&ctx->d_res_util, &ctx->d_res_power, &ctx->d_idx_util, &ctx->d_idx_power}) CU(b->release());
   ctx->idx_ld = 0;
@@ -1326,19 +1330,17 @@ int gpr_resident_init(gpr_ctx* ctx, uint32_t P, uint32_t G, uint32_t T, uint32_t
 int gpr_resident_reindex(gpr_ctx* ctx) {
   if (!ctx) return GPR_E_INVALID;
   GPR_TRY
+  if (const int rc = enter(ctx)) return rc;
   if (!ctx->d_res_util) return fail(ctx, GPR_E_STATE, "no resident window (gpr_resident_init)");
   if (!ctx->d_idx_util) return GPR_OK;  // no index to maintain
-  CU(cudaSetDevice(ctx->device));
-  ctx->last_was_reduce = false;
   const size_t rows = (size_t)ctx->res_P * ctx->res_G;
   const uint32_t grid = gpr::ring_grid(rows, ctx->sm_count);
-  gpr::k_reindex<<<grid, gpr::kRingThreads, 0, ctx->stream>>>(ctx->d_res_util, (uint32_t)rows, ctx->res_T,
-                                                             ctx->d_idx_util, ctx->idx_ld);
-  if (ctx->d_res_power)
-    gpr::k_reindex<<<grid, gpr::kRingThreads, 0, ctx->stream>>>(ctx->d_res_power, (uint32_t)rows, ctx->res_T,
-                                                               ctx->d_idx_power, ctx->idx_ld);
-  ctx->launches += ctx->d_res_power ? 2 : 1;
-  CU(cudaGetLastError());
+  int rc = launch(ctx, gpr::k_reindex, grid, gpr::kRingThreads, 0, false, ctx->d_res_util, (uint32_t)rows, ctx->res_T,
+                  ctx->d_idx_util, ctx->idx_ld);
+  if (rc == GPR_OK && ctx->d_res_power)
+    rc = launch(ctx, gpr::k_reindex, grid, gpr::kRingThreads, 0, false, ctx->d_res_power, (uint32_t)rows, ctx->res_T,
+                ctx->d_idx_power, ctx->idx_ld);
+  if (rc != GPR_OK) return rc;
   CU(cudaStreamSynchronize(ctx->stream));
   ctx->idx_stale = false;
   return GPR_OK;
@@ -1349,13 +1351,12 @@ int gpr_append(gpr_ctx* ctx, const float* util_cols, const float* power_cols, ui
                uint64_t row_stride, int32_t mem_kind) {
   if (!ctx) return GPR_E_INVALID;
   GPR_TRY
+  if (const int rc = enter(ctx)) return rc;
   if (!ctx->d_res_util) return fail(ctx, GPR_E_STATE, "no resident window (gpr_resident_init)");
   if (n_new == 0) return GPR_OK;
   if (!util_cols) return fail(ctx, GPR_E_INVALID, "util_cols is NULL");
-  ctx->last_was_reduce = false;
   if (mem_kind != GPR_MEM_HOST && mem_kind != GPR_MEM_DEVICE)
     return fail(ctx, GPR_E_INVALID, "bad mem_kind %d", mem_kind);
-  CU(cudaSetDevice(ctx->device));
   const uint32_t T = ctx->res_T;
   const size_t rows = (size_t)ctx->res_P * ctx->res_G;
   uint64_t ld = row_stride ? row_stride : n_new;
@@ -1370,11 +1371,11 @@ int gpr_append(gpr_ctx* ctx, const float* util_cols, const float* power_cols, ui
   for (int pl = 0; pl < 2; ++pl) {
     const gpr::RingLaunch what = gpr::append_launch(planes_out[pl] != nullptr, planes_in[pl] != nullptr);
     if (what == gpr::kRingNone) continue;
+    int rc;
     if (what == gpr::kRingOpen) {  // no columns for this plane: its new buckets hold no sample
-      gpr::k_open<<<grid, gpr::kRingThreads, 0, ctx->stream>>>(planes_out[pl], (uint32_t)rows, T, sp.start, sp.n,
-                                                               planes_idx[pl], ctx->idx_ld);
-      ctx->launches++;
-      CU(cudaGetLastError());
+      if ((rc = launch(ctx, gpr::k_open, grid, gpr::kRingThreads, 0, false, planes_out[pl], (uint32_t)rows, T, sp.start,
+                       sp.n, planes_idx[pl], ctx->idx_ld)) != GPR_OK)
+        return rc;
       continue;
     }
     const float* src = planes_in[pl] + sp.src_col;
@@ -1390,10 +1391,9 @@ int gpr_append(gpr_ctx* ctx, const float* util_cols, const float* power_cols, ui
       src = ctx->d_cols;
       ld_dev = n_eff;
     }
-    gpr::k_append<<<grid, gpr::kRingThreads, 0, ctx->stream>>>(planes_out[pl], src, (uint32_t)rows, T, sp.start,
-                                                               sp.n, ld_dev, planes_idx[pl], ctx->idx_ld);
-    ctx->launches++;
-    CU(cudaGetLastError());
+    if ((rc = launch(ctx, gpr::k_append, grid, gpr::kRingThreads, 0, false, planes_out[pl], src, (uint32_t)rows, T,
+                     sp.start, sp.n, ld_dev, planes_idx[pl], ctx->idx_ld)) != GPR_OK)
+      return rc;
   }
   ctx->res_head = sp.next_head;
   CU(cudaStreamSynchronize(ctx->stream));
@@ -1410,11 +1410,11 @@ static int remap_check_device(gpr_ctx* ctx, const uint32_t* src_rows, uint32_t n
   unsigned int* d = ctx->d_remap_check;
   CU(cudaMemsetAsync(d + 1, 0, 2 * words * sizeof(unsigned int), ctx->stream));
   CU(cudaMemcpyAsync(d, &n_new, sizeof n_new, cudaMemcpyHostToDevice, ctx->stream));
-  const uint32_t blocks = std::max(1u, std::min((n_new + 255u) / 256u, (uint32_t)ctx->sm_count * 8u));
+  const uint32_t blocks = capped_grid(ctx, n_new, 256, 8);
   for (int pass = 0; pass < 2; ++pass) {
-    gpr::k_remap_check<<<blocks, 256, 0, ctx->stream>>>(src_rows, n_new, n_old, d + 1, d + 1 + words, d, pass);
-    ctx->launches++;
-    CU(cudaGetLastError());
+    const int rc = launch(ctx, gpr::k_remap_check, blocks, 256, 0, false, src_rows, n_new, n_old, d + 1, d + 1 + words,
+                          d, pass);
+    if (rc != GPR_OK) return rc;
   }
   CU(cudaMemcpyAsync(first, d, sizeof *first, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
@@ -1434,11 +1434,10 @@ static int remap_build(gpr_ctx* ctx, const uint32_t* map, uint32_t n_rows) {
   for (int k = 0; k < 4; ++k) {
     if (!*cur[k]) continue;
     CU(ctx->d_res_next[k].alloc((size_t)n_rows * len[k]));
-    gpr::k_remap_rows<<<grid, gpr::kRingThreads, 0, ctx->stream>>>(reinterpret_cast<uint32_t*>(ctx->d_res_next[k].p),
-                                                                  reinterpret_cast<const uint32_t*>(cur[k]->p), map,
-                                                                  n_rows, len[k]);
-    ctx->launches++;
-    CU(cudaGetLastError());
+    const int rc = launch(ctx, gpr::k_remap_rows, grid, gpr::kRingThreads, 0, false,
+                          reinterpret_cast<uint32_t*>(ctx->d_res_next[k].p), reinterpret_cast<const uint32_t*>(cur[k]->p),
+                          map, n_rows, len[k]);
+    if (rc != GPR_OK) return rc;
   }
   CU(cudaStreamSynchronize(ctx->stream));
   return GPR_OK;
@@ -1448,13 +1447,12 @@ int gpr_resident_remap(gpr_ctx* ctx, uint32_t n_pods, uint32_t n_gpus, const uin
   if (!ctx) return GPR_E_INVALID;
   GPR_TRY
   NvtxRange nvtx_range("gpr_resident_remap");
+  if (const int rc = enter(ctx)) return rc;
   if (!ctx->d_res_util) return fail(ctx, GPR_E_STATE, "no resident window (gpr_resident_init)");
   if (n_pods == 0 || n_gpus == 0) return fail(ctx, GPR_E_INVALID, "empty resident window");
   if ((uint64_t)n_pods * n_gpus > 0x7fffffffull) return fail(ctx, GPR_E_INVALID, "too many series");
   if (!src_rows) return fail(ctx, GPR_E_INVALID, "src_rows is NULL");
   if (mem_kind != GPR_MEM_HOST && mem_kind != GPR_MEM_DEVICE) return fail(ctx, GPR_E_INVALID, "bad mem_kind %d", mem_kind);
-  CU(cudaSetDevice(ctx->device));
-  ctx->last_was_reduce = false;
   const uint32_t n_new = n_pods * n_gpus, n_old = ctx->res_P * ctx->res_G;
   // ---- the map is checked before the new ring is allocated or anything of the ring is written
   uint32_t first = n_new, src = 0;
@@ -1512,10 +1510,9 @@ int gpr_resident_head(gpr_ctx* ctx, uint32_t* head) {
 int gpr_resident_advance(gpr_ctx* ctx, uint32_t n_new) {
   if (!ctx) return GPR_E_INVALID;
   GPR_TRY
+  if (const int rc = enter(ctx)) return rc;
   if (!ctx->d_res_util) return fail(ctx, GPR_E_STATE, "no resident window (gpr_resident_init)");
   if (n_new == 0) return GPR_OK;
-  CU(cudaSetDevice(ctx->device));
-  ctx->last_was_reduce = false;
   const uint32_t T = ctx->res_T;
   const size_t rows = (size_t)ctx->res_P * ctx->res_G;
   const gpr::RingSpan sp = gpr::ring_span(ctx->res_head, n_new, T);
@@ -1525,20 +1522,17 @@ int gpr_resident_advance(gpr_ctx* ctx, uint32_t n_new) {
     float* pl = planes[k];
     const gpr::RingLaunch what = gpr::advance_launch(pl != nullptr, planes_idx[k] != nullptr);
     if (what == gpr::kRingNone) continue;
+    int rc = GPR_OK;
     if (what == gpr::kRingOpen) {  // the opened buckets' old samples leave the index too
-      gpr::k_open<<<gpr::ring_grid(rows, ctx->sm_count), gpr::kRingThreads, 0, ctx->stream>>>(
-          pl, (uint32_t)rows, T, sp.start, sp.n, planes_idx[k], ctx->idx_ld);
-      ctx->launches++;
-      CU(cudaGetLastError());
+      rc = launch(ctx, gpr::k_open, gpr::ring_grid(rows, ctx->sm_count), gpr::kRingThreads, 0, false, pl, (uint32_t)rows,
+                  T, sp.start, sp.n, planes_idx[k], ctx->idx_ld);
     } else if (n_new >= T) {
       CU(cudaMemsetAsync(pl, 0xFF, rows * (size_t)T * sizeof(float), ctx->stream));
     } else {
-      const uint64_t total = (uint64_t)rows * n_new;
-      const uint32_t grid = (uint32_t)std::min<uint64_t>((total + 255) / 256, (uint64_t)ctx->sm_count * 16);
-      gpr::text::k_fill_columns<<<grid, 256, 0, ctx->stream>>>(pl, (uint32_t)rows, T, T, ctx->res_head, n_new);
-      ctx->launches++;
-      CU(cudaGetLastError());
+      rc = launch(ctx, gpr::text::k_fill_columns, capped_grid(ctx, (uint64_t)rows * n_new, 256, 16), 256, 0, false, pl,
+                  (uint32_t)rows, T, T, ctx->res_head, n_new);
     }
+    if (rc != GPR_OK) return rc;
   }
   ctx->res_head = sp.next_head;
   CU(cudaStreamSynchronize(ctx->stream));
@@ -1564,12 +1558,12 @@ int gpr_comm_unique_id(void* id128) {
 int gpr_comm_init(gpr_ctx* ctx, const void* id128, int rank, int world) {
   if (!ctx) return GPR_E_INVALID;
   GPR_TRY
+  if (const int rc = enter(ctx)) return rc;
   if (!id128 || world < 1 || rank < 0 || rank >= world)
     return fail(ctx, GPR_E_INVALID, "bad communicator arguments (rank %d world %d)", rank, world);
   if (ctx->comm) return fail(ctx, GPR_E_STATE, "communicator already attached");
   char err[256];
   if (!load_nccl(err, sizeof err)) return fail(ctx, GPR_E_NCCL, "%s", err);
-  CU(cudaSetDevice(ctx->device));
   ncclUniqueId id;
   memcpy(&id, id128, sizeof id);
   NC(g_nccl.CommInitRank(&ctx->comm, world, id, rank));
@@ -1581,8 +1575,8 @@ int gpr_comm_init(gpr_ctx* ctx, const void* id128, int rank, int world) {
 int gpr_comm_destroy(gpr_ctx* ctx) {
   if (!ctx) return GPR_E_INVALID;
   GPR_TRY
+  if (const int rc = enter(ctx)) return rc;
   if (ctx->comm) {
-    CU(cudaSetDevice(ctx->device));
     CU(cudaStreamSynchronize(ctx->stream));
     NC(g_nccl.CommDestroy(ctx->comm));
     ctx->comm = nullptr;
@@ -1597,6 +1591,7 @@ int gpr_comm_destroy(gpr_ctx* ctx) {
 int gpr_p2p_init(gpr_ctx* ctx, int rank, int world, uint32_t max_pods_per_rank, void* handle64) {
   if (!ctx) return GPR_E_INVALID;
   GPR_TRY
+  if (const int rc = enter(ctx)) return rc;
   if (!handle64 || world < 2 || world > gpr::kMaxPeers || rank < 0 || rank >= world)
     return fail(ctx, GPR_E_INVALID, "bad p2p arguments (rank %d world %d, at most %d ranks)", rank, world,
                 gpr::kMaxPeers);
@@ -1604,7 +1599,6 @@ int gpr_p2p_init(gpr_ctx* ctx, int rank, int world, uint32_t max_pods_per_rank, 
   if (ctx->comm && (ctx->rank != rank || ctx->world != world))
     return fail(ctx, GPR_E_INVALID, "rank/world differ from the NCCL communicator's");
   static_assert(sizeof(cudaIpcMemHandle_t) == GPR_P2P_HANDLE_BYTES, "cudaIpcMemHandle_t size");
-  CU(cudaSetDevice(ctx->device));
   const uint32_t w_max = (max_pods_per_rank + 31u) / 32u;
   ctx->p2p_stride = 2u * std::max<uint32_t>(w_max, 1u);
   const size_t gather_bytes = ((size_t)world * ctx->p2p_stride * 4u + 255u) & ~(size_t)255u;
@@ -1627,10 +1621,10 @@ int gpr_p2p_init(gpr_ctx* ctx, int rank, int world, uint32_t max_pods_per_rank, 
 int gpr_p2p_attach(gpr_ctx* ctx, const void* handles) {
   if (!ctx) return GPR_E_INVALID;
   GPR_TRY
+  if (const int rc = enter(ctx)) return rc;
   if (!handles) return fail(ctx, GPR_E_INVALID, "handles is NULL");
   if (!ctx->p2p_block) return fail(ctx, GPR_E_STATE, "call gpr_p2p_init first");
   if (ctx->p2p_ready) return fail(ctx, GPR_E_STATE, "p2p exchange already attached");
-  CU(cudaSetDevice(ctx->device));
   for (int r = 0; r < ctx->world; ++r) {
     if (r == ctx->rank) {
       ctx->p2p_peer[r] = ctx->p2p_block;
@@ -1650,7 +1644,7 @@ int gpr_p2p_attach(gpr_ctx* ctx, const void* handles) {
 // ---- memory helpers -----------------------------------------------------------------------------
 int gpr_host_alloc(gpr_ctx* ctx, size_t bytes, void** out) {
   if (!ctx || !out) return GPR_E_INVALID;
-  CU(cudaSetDevice(ctx->device));
+  if (const int rc = enter(ctx)) return rc;
   CU(cudaMallocHost(out, bytes ? bytes : 1));
   return GPR_OK;
 }
@@ -1661,23 +1655,22 @@ int gpr_host_free(gpr_ctx* ctx, void* p) {
 }
 int gpr_device_alloc(gpr_ctx* ctx, size_t bytes, void** out) {
   if (!ctx || !out) return GPR_E_INVALID;
-  CU(cudaSetDevice(ctx->device));
+  if (const int rc = enter(ctx)) return rc;
   CU(cudaMalloc(out, bytes ? bytes : 1));
   return GPR_OK;
 }
 int gpr_device_free(gpr_ctx* ctx, void* p) {
   if (!ctx) return GPR_E_INVALID;
-  CU(cudaSetDevice(ctx->device));
+  if (const int rc = enter(ctx)) return rc;
   if (p) CU(cudaFree(p));
   return GPR_OK;
 }
 int gpr_memcpy(gpr_ctx* ctx, void* dst, const void* src, size_t bytes, int32_t dst_kind,
                int32_t src_kind) {
   if (!ctx) return GPR_E_INVALID;
+  if (const int rc = enter(ctx)) return rc;
   if (bytes == 0) return GPR_OK;
   if (!dst || !src) return fail(ctx, GPR_E_INVALID, "NULL pointer in gpr_memcpy");
-  ctx->last_was_reduce = false;
-  CU(cudaSetDevice(ctx->device));
   cudaMemcpyKind k = dst_kind == GPR_MEM_DEVICE
                          ? (src_kind == GPR_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice)
                          : (src_kind == GPR_MEM_DEVICE ? cudaMemcpyDeviceToHost : cudaMemcpyHostToHost);
@@ -1689,8 +1682,7 @@ int gpr_memcpy(gpr_ctx* ctx, void* dst, const void* src, size_t bytes, int32_t d
 // ---- measurement support --------------------------------------------------------------------------
 int gpr_timer_begin(gpr_ctx* ctx) {
   if (!ctx) return GPR_E_INVALID;
-  ctx->last_was_reduce = false;
-  CU(cudaSetDevice(ctx->device));
+  if (const int rc = enter(ctx)) return rc;
   // rendezvous first, then the start event: with an exchange attached the timed regions of all ranks
   // begin within an NVLink round trip of each other, whatever the skew between their host threads
   gpr::RendezvousParams q;
@@ -1710,9 +1702,7 @@ int gpr_timer_begin(gpr_ctx* ctx) {
     CU(ctx->d_bits.grow(ctx->stream, 4));
     NC(g_nccl.AllGather(ctx->d_bits, ctx->d_gather, 1, ncclUint32, ctx->comm, ctx->stream));
   }
-  gpr::k_rendezvous<<<1, 32, 0, ctx->stream>>>(q);
-  ctx->launches++;
-  CU(cudaGetLastError());
+  if (const int rc = launch(ctx, gpr::k_rendezvous, 1, 32, 0, false, q)) return rc;
   CU(cudaEventRecord(ctx->ev_t0, ctx->stream));
   return GPR_OK;
 }
@@ -1739,8 +1729,7 @@ int gpr_p2p_debug(gpr_ctx* ctx, int32_t mode) {
 }
 int gpr_timer_end(gpr_ctx* ctx, double* ms) {
   if (!ctx || !ms) return GPR_E_INVALID;
-  ctx->last_was_reduce = false;
-  CU(cudaSetDevice(ctx->device));
+  if (const int rc = enter(ctx)) return rc;
   CU(cudaEventRecord(ctx->ev_t1, ctx->stream));
   CU(cudaEventSynchronize(ctx->ev_t1));
   float f = 0.f;
@@ -1750,8 +1739,7 @@ int gpr_timer_end(gpr_ctx* ctx, double* ms) {
 }
 int gpr_flush_l2(gpr_ctx* ctx) {
   if (!ctx) return GPR_E_INVALID;
-  ctx->last_was_reduce = false;
-  CU(cudaSetDevice(ctx->device));
+  if (const int rc = enter(ctx)) return rc;
   CU(ctx->d_flush.alloc_once(std::max<size_t>(ctx->l2_bytes * 2, (size_t)256 << 20)));
   CU(cudaMemsetAsync(ctx->d_flush, 0x5a, ctx->d_flush.cap, ctx->stream));
   return GPR_OK;
@@ -1783,11 +1771,11 @@ int gpr_text_scan_begin(gpr_ctx* ctx, int32_t slot, const char* text, uint64_t n
   if (!ctx) return GPR_E_INVALID;
   GPR_TRY
   NvtxRange nvtx_range("gpr_text_scan_begin");
+  if (const int rc = enter(ctx)) return rc;
   if (slot < 0 || slot > 2) return fail(ctx, GPR_E_INVALID, "text slot %d (0..2)", slot);
   if (!text && n_bytes) return fail(ctx, GPR_E_INVALID, "text is NULL");
   if (mem_kind != GPR_MEM_HOST && mem_kind != GPR_MEM_DEVICE) return fail(ctx, GPR_E_INVALID, "bad mem_kind %d", mem_kind);
   scan_pipe_abort(ctx);  // an unfinished scan is dropped
-  CU(cudaSetDevice(ctx->device));
   CU(ctx->d_text[slot].grow(ctx->stream, (size_t)n_bytes + gpr::text::kTextPad));
   constexpr int NT = gpr_ctx::kUpThreads, NS = gpr_ctx::kUpSlots, NB = gpr_ctx::kMarkBlocks;
   CU(ctx->h_mark_blocks.alloc_once((size_t)NB * kBlockWords, cudaHostAllocMapped));
@@ -1799,19 +1787,13 @@ int gpr_text_scan_begin(gpr_ctx* ctx, int32_t slot, const char* text, uint64_t n
   }
   uint8_t* d = ctx->d_text[slot];
   ctx->text_n[slot] = n_bytes;
-  ctx->last_was_reduce = false;
   // the zero pad behind the text, and everything earlier on the context's stream that may still read the buffer
   CU(cudaMemsetAsync(d + n_bytes, 0, gpr::text::kTextPad, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   ScanPipe* sp = new ScanPipe();
   sp->slot = slot, sp->src = text, sp->dst = d, sp->n = n_bytes, sp->src_kind = mem_kind;
   for (auto& r : sp->recorded) r.store(0);
-  if (mem_kind == GPR_MEM_HOST && n_bytes) {
-    cudaPointerAttributes at;
-    const bool pinned = cudaPointerGetAttributes(&at, text) == cudaSuccess && at.type == cudaMemoryTypeHost;
-    (void)cudaGetLastError();  // an unregistered pointer may leave an error code behind
-    sp->staged = !pinned;
-  }
+  sp->staged = mem_kind == GPR_MEM_HOST && n_bytes && !host_pinned(text, nullptr);
   sp->chunk = sp->staged ? ctx->up_chunk : gpr_ctx::kPinnedChunk;
   sp->n_chunks = (n_bytes + sp->chunk - 1) / sp->chunk;
   sp->unit = std::min<uint64_t>(sp->chunk, gpr_ctx::kScanUnit);
@@ -1844,6 +1826,7 @@ int gpr_text_scan_next(gpr_ctx* ctx, uint64_t* opens, uint64_t* closes, uint64_t
                        uint64_t* bytes_done, int32_t* more) {
   if (!ctx) return GPR_E_INVALID;
   GPR_TRY
+  if (const int rc = enter(ctx)) return rc;
   if (!n_opens || !n_closes || !bytes_done || !more || (cap && (!opens || !closes)))
     return fail(ctx, GPR_E_INVALID, "output pointers are NULL");
   ScanPipe* sp = ctx->pipe;
@@ -1859,7 +1842,6 @@ int gpr_text_scan_next(gpr_ctx* ctx, uint64_t* opens, uint64_t* closes, uint64_t
     if (sp->error.load() || sp->stop.load()) return scan_pipe_finish(ctx, false) != GPR_OK ? GPR_E_CUDA : fail(ctx, GPR_E_CUDA, "text upload stopped");
     std::this_thread::yield();
   }
-  CU(cudaSetDevice(ctx->device));
   cudaError_t e = cudaEventSynchronize(ctx->mark_event[u % NB]);
   if (e != cudaSuccess) {
     (void)scan_pipe_finish(ctx, false);
@@ -1900,6 +1882,7 @@ int gpr_text_scan(gpr_ctx* ctx, int32_t slot, const char* text, uint64_t n_bytes
   if (!ctx) return GPR_E_INVALID;
   GPR_TRY
   NvtxRange nvtx_range("gpr_text_scan");
+  if (const int rc = enter(ctx)) return rc;
   if (!n_opens || !n_closes || (cap && (!opens || !closes))) return fail(ctx, GPR_E_INVALID, "output arrays are NULL");
   int rc = gpr_text_scan_begin(ctx, slot, text, n_bytes, mem_kind);
   if (rc != GPR_OK) return rc;
@@ -1930,7 +1913,9 @@ int gpr_text_scan(gpr_ctx* ctx, int32_t slot, const char* text, uint64_t n_bytes
 int gpr_text_parse(gpr_ctx* ctx, int32_t slot, gpr_text_span* spans, uint32_t n_spans, const gpr_text_grid* grid,
                    int32_t plane) {
   if (!ctx) return GPR_E_INVALID;
+  GPR_TRY
   NvtxRange nvtx_range("gpr_text_parse");
+  if (const int rc = enter(ctx)) return rc;
   if (!grid || grid->struct_size != sizeof(gpr_text_grid)) return fail(ctx, GPR_E_INVALID, "grid is NULL / struct_size mismatch");
   if (slot < 0 || slot > 2 || plane < 0 || plane > 1) return fail(ctx, GPR_E_INVALID, "bad slot %d / plane %d", slot, plane);
   if (!ctx->d_text[slot]) return fail(ctx, GPR_E_STATE, "no text in slot %d (gpr_text_scan)", slot);
@@ -1946,29 +1931,25 @@ int gpr_text_parse(gpr_ctx* ctx, int32_t slot, gpr_text_span* spans, uint32_t n_
     spans[i].flags &= GPR_SPAN_SHARED;
     spans[i].n_in = spans[i].n_oow = spans[i].n_tiny = 0;
   }
-  CU(cudaSetDevice(ctx->device));
   float* pl = nullptr;
   gpr::text::Grid g;
-  if ((rc = text_destination(ctx, grid, plane, &g, &pl)) != GPR_OK) return rc;
-  if ((rc = open_destination(ctx, grid, pl)) != GPR_OK) return rc;
+  if ((rc = open_destination(ctx, grid, plane, &g, &pl)) != GPR_OK) return rc;
   CU(ctx->d_spans.grow(ctx->stream, (size_t)n_spans + 1));
-  ctx->last_was_reduce = false;
   if (n_spans && n) {
     CU(cudaMemcpyAsync(ctx->d_spans, spans, (size_t)n_spans * sizeof(gpr_text_span), cudaMemcpyHostToDevice,
                        ctx->stream));
     constexpr int kWarps = 4;
     const uint64_t tiles = (n + gpr::text::kTileBytes - 1) / gpr::text::kTileBytes;
-    const uint32_t blocks = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((tiles + kWarps - 1) / kWarps,
-                                                                                (uint64_t)ctx->sm_count * ctx->parse_ctas_per_sm));
-    gpr::text::k_text_parse<kWarps><<<blocks, kWarps * 32, gpr::text::text_parse_smem<kWarps>(), ctx->stream>>>(
-        ctx->d_text[slot], n, n + gpr::text::kTextPad, ctx->d_spans, n_spans, g, pl);
-    ctx->launches++;
-    CU(cudaGetLastError());
+    if ((rc = launch(ctx, gpr::text::k_text_parse<kWarps>, capped_grid(ctx, tiles, kWarps, ctx->parse_ctas_per_sm),
+                     kWarps * 32, gpr::text::text_parse_smem<kWarps>(), false, ctx->d_text[slot], n,
+                     n + gpr::text::kTextPad, ctx->d_spans, n_spans, g, pl)) != GPR_OK)
+      return rc;
     CU(cudaMemcpyAsync(spans, ctx->d_spans, (size_t)n_spans * sizeof(gpr_text_span), cudaMemcpyDeviceToHost,
                        ctx->stream));
   }
   CU(cudaStreamSynchronize(ctx->stream));
   return GPR_OK;
+  GPR_CATCH(ctx)
 }
 
 int gpr_text_planes(gpr_ctx* ctx, float** util, float** power) {
@@ -1978,30 +1959,78 @@ int gpr_text_planes(gpr_ctx* ctx, float** util, float** power) {
   return GPR_OK;
 }
 
-// ---- decoded samples (gpr_samples.cuh) ---------------------------------------------------------------
+// ---- decoded samples (gpr_samples.cuh) and Prometheus XOR chunks (gpr_chunks.cuh) --------------------------------
+// Both merges check a batch the same way before anything is written, then merge into gpr_text_parse's destination.
 static_assert(sizeof(gpr_sample_stats) == 24, "gpr_sample_stats");
 
-static int launch_scatter(gpr_ctx* ctx, const gpr::samples::ScatterArgs& a, bool vec) {
+// The arguments of a batch (gpr_sample_batch or gpr_chunk_batch) and of its grid
+extern "C++" {  // (templates)
+template <typename Batch>
+static int check_batch_args(gpr_ctx* ctx, const Batch* batch, const gpr_text_grid* grid, int32_t plane) {
+  if (!batch || batch->struct_size != sizeof(Batch)) return fail(ctx, GPR_E_INVALID, "batch is NULL / struct_size mismatch");
+  if (!grid || grid->struct_size != sizeof(gpr_text_grid)) return fail(ctx, GPR_E_INVALID, "grid is NULL / struct_size mismatch");
+  if (plane < 0 || plane > 1) return fail(ctx, GPR_E_INVALID, "bad plane %d", plane);
+  if (batch->mem_kind != GPR_MEM_HOST && batch->mem_kind != GPR_MEM_DEVICE)
+    return fail(ctx, GPR_E_INVALID, "bad mem_kind %d", batch->mem_kind);
+  return check_grid(ctx, grid);
+}
+}  // extern "C++"
+
+// A batch's series index, offsets[n_series + 1] (into its samples, or its chunks) and rows[n_series], checked where it
+// is: on the host, or on the device by k_samples_check.  *bad gets the series_faults() bits of every series and *total
+// offsets[n_series].  (The first use of a batch's scratch d_sstats, which is allocated here.)
+static int check_series_index(gpr_ctx* ctx, const uint64_t* offsets, const uint32_t* rows, uint32_t S, bool host,
+                              uint32_t n_rows, uint32_t* bad, uint64_t* total) {
   namespace gs = gpr::samples;
-  const uint64_t chunks = (a.end - a.base + gs::kChunk - 1) / gs::kChunk;
-  const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(chunks, (uint64_t)ctx->sm_count * 8));
-  if (vec) gs::k_samples_scatter<true><<<grid, gs::kThreads, 0, ctx->stream>>>(a);
-  else gs::k_samples_scatter<false><<<grid, gs::kThreads, 0, ctx->stream>>>(a);
-  ctx->launches++;
-  CU(cudaGetLastError());
+  CU(ctx->d_sstats.alloc_once(5));
+  if (host) {
+    *bad = 0;
+    for (uint32_t s = 0; s < std::max(S, 1u); ++s) *bad |= gs::series_faults(offsets, rows, S, s, n_rows);
+    *total = offsets[S];
+    return GPR_OK;
+  }
+  unsigned long long back[2] = {0, 0};  // the check word, offsets[n_series]
+  unsigned int* d_bad = reinterpret_cast<unsigned int*>(ctx->d_sstats + 2);
+  CU(cudaMemsetAsync(d_bad, 0, sizeof(unsigned long long), ctx->stream));
+  const int rc = launch(ctx, gs::k_samples_check, capped_grid(ctx, std::max(S, 1u), 256, 8), 256, 0, false, offsets, rows,
+                        S, n_rows, d_bad);
+  if (rc != GPR_OK) return rc;
+  CU(cudaMemcpyAsync(&back[0], d_bad, sizeof back[0], cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(&back[1], offsets + S, sizeof back[1], cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  *bad = (uint32_t)back[0], *total = back[1];
   return GPR_OK;
 }
 
-// Whether both host arrays are pinned (registered with CUDA); pageable ones go up through pinned staging.
-static bool host_pinned(const void* a, const void* b) {
-  bool pinned = true;
-  for (const void* p : {a, b}) {
-    if (!p) continue;
-    cudaPointerAttributes at;
-    pinned = pinned && cudaPointerGetAttributes(&at, p) == cudaSuccess && at.type == cudaMemoryTypeHost;
-    (void)cudaGetLastError();  // an unregistered pointer may leave an error code behind
-  }
-  return pinned;
+// a host batch's series index, uploaded whole (12 B per series)
+static int upload_series_index(gpr_ctx* ctx, const uint64_t* offsets, const uint32_t* rows, uint32_t S) {
+  CU(ctx->d_soffsets.grow(ctx->stream, (size_t)S + 1));
+  CU(ctx->d_srows.grow(ctx->stream, (size_t)S + 1));
+  CU(cudaMemcpyAsync(ctx->d_soffsets, offsets, ((size_t)S + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(ctx->d_srows, rows, (size_t)S * 4, cudaMemcpyHostToDevice, ctx->stream));
+  return GPR_OK;
+}
+
+// rc, after the stream has drained if it is an error: the staging buffers of a failed step may still be read
+static int drain_on_error(gpr_ctx* ctx, int rc) {
+  if (rc != GPR_OK) (void)cudaStreamSynchronize(ctx->stream);
+  return rc;
+}
+
+// The end of a merge whose work is enqueued with status rc: n_in and the merge's counts go to *stats.
+static int finish_merge(gpr_ctx* ctx, int rc, uint64_t n_in, gpr_sample_stats* stats) {
+  if (drain_on_error(ctx, rc) != GPR_OK) return rc;
+  unsigned long long counts[2] = {0, 0};
+  CU(cudaMemcpyAsync(counts, ctx->d_sstats, sizeof counts, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  if (stats) stats->n_in = n_in, stats->n_oow = counts[0], stats->n_tiny = counts[1];
+  return GPR_OK;
+}
+
+static int launch_scatter(gpr_ctx* ctx, const gpr::samples::ScatterArgs& a, bool vec) {
+  namespace gs = gpr::samples;
+  return launch(ctx, vec ? gs::k_samples_scatter<true> : gs::k_samples_scatter<false>,
+                capped_grid(ctx, a.end - a.base, gs::kChunk, 8), gs::kThreads, 0, false, a);
 }
 
 // The staging of a host batch (gpr_samples_scatter, gpr_chunks_scatter): two device buffers of 2 x kStageHalf bytes
@@ -2057,13 +2086,10 @@ static int stage_piece(gpr_ctx* ctx, uint64_t k, bool pinned, const void* const 
 static int scatter_host_pieces(gpr_ctx* ctx, const gpr_sample_batch* batch, uint64_t total, gpr::samples::ScatterArgs a) {
   namespace gs = gpr::samples;
   const uint32_t S = batch->n_series;
-  CU(ctx->d_soffsets.grow(ctx->stream, (size_t)S + 1));
-  CU(ctx->d_srows.grow(ctx->stream, (size_t)S + 1));
-  CU(cudaMemcpyAsync(ctx->d_soffsets, batch->offsets, ((size_t)S + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
-  CU(cudaMemcpyAsync(ctx->d_srows, batch->rows, (size_t)S * 4, cudaMemcpyHostToDevice, ctx->stream));
+  int rc;
+  if ((rc = upload_series_index(ctx, batch->offsets, batch->rows, S)) != GPR_OK) return rc;
   a.offsets = ctx->d_soffsets, a.rows = ctx->d_srows;
   const bool pinned = host_pinned(batch->ts_ms, batch->values);
-  int rc;
   if ((rc = open_staging(ctx, pinned)) != GPR_OK) return rc;
   uint64_t k = 0;
   return gs::for_each_piece(batch->offsets, S, total, gs::kHostPiece, [&](const gs::Piece& p) -> int {
@@ -2085,66 +2111,34 @@ int gpr_samples_scatter(gpr_ctx* ctx, const gpr_sample_batch* batch, const gpr_t
   GPR_TRY
   NvtxRange nvtx_range("gpr_samples_scatter");
   namespace gs = gpr::samples;
-  if (!batch || batch->struct_size != sizeof(gpr_sample_batch))
-    return fail(ctx, GPR_E_INVALID, "batch is NULL / struct_size mismatch");
-  if (!grid || grid->struct_size != sizeof(gpr_text_grid)) return fail(ctx, GPR_E_INVALID, "grid is NULL / struct_size mismatch");
-  if (plane < 0 || plane > 1) return fail(ctx, GPR_E_INVALID, "bad plane %d", plane);
-  if (batch->mem_kind != GPR_MEM_HOST && batch->mem_kind != GPR_MEM_DEVICE)
-    return fail(ctx, GPR_E_INVALID, "bad mem_kind %d", batch->mem_kind);
   int rc;
-  if ((rc = check_grid(ctx, grid)) != GPR_OK) return rc;
+  if ((rc = enter(ctx)) != GPR_OK || (rc = check_batch_args(ctx, batch, grid, plane)) != GPR_OK) return rc;
   const uint32_t S = batch->n_series;
+  const bool host = batch->mem_kind == GPR_MEM_HOST;
   if (!batch->offsets || (S && !batch->rows)) return fail(ctx, GPR_E_INVALID, "offsets / rows is NULL");
-  CU(cudaSetDevice(ctx->device));
-  ctx->last_was_reduce = false;
-  CU(ctx->d_sstats.alloc_once(4));
   // ---- the batch is checked before anything is written
   uint32_t bad = 0;
   uint64_t total = 0;
-  if (batch->mem_kind == GPR_MEM_HOST) {
-    for (uint32_t s = 0; s < std::max(S, 1u); ++s) bad |= gs::series_faults(batch->offsets, batch->rows, S, s, grid->n_rows);
-    total = batch->offsets[S];
-  } else {
-    unsigned long long back[2] = {0, 0};  // the check word, offsets[n_series]
-    CU(cudaMemsetAsync(ctx->d_sstats + 2, 0, sizeof(unsigned long long), ctx->stream));
-    const uint32_t blocks = std::max(1u, std::min((std::max(S, 1u) + 255u) / 256u, (uint32_t)ctx->sm_count * 8u));
-    gs::k_samples_check<<<blocks, 256, 0, ctx->stream>>>(batch->offsets, batch->rows, S, grid->n_rows,
-                                                         reinterpret_cast<unsigned int*>(ctx->d_sstats + 2));
-    ctx->launches++;
-    CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(&back[0], ctx->d_sstats + 2, sizeof back[0], cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaMemcpyAsync(&back[1], batch->offsets + S, sizeof back[1], cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
-    bad = (uint32_t)back[0], total = back[1];
-  }
+  if ((rc = check_series_index(ctx, batch->offsets, batch->rows, S, host, grid->n_rows, &bad, &total)) != GPR_OK)
+    return rc;
   if (bad & gs::kBadStart) return fail(ctx, GPR_E_INVALID, "gpr_sample_batch: offsets[0] != 0");
   if (bad & gs::kBadOrder) return fail(ctx, GPR_E_INVALID, "gpr_sample_batch: offsets decrease");
   if (bad & gs::kBadRow) return fail(ctx, GPR_E_INVALID, "gpr_sample_batch: a row >= grid.n_rows (%u)", grid->n_rows);
   if (total && (!batch->ts_ms || !batch->values)) return fail(ctx, GPR_E_INVALID, "ts_ms / values is NULL");
   // ---- the destination, then the merge
-  float* pl = nullptr;
   gs::ScatterArgs a;
   memset(&a, 0, sizeof a);
-  if ((rc = text_destination(ctx, grid, plane, &a.g, &pl)) != GPR_OK) return rc;
-  if ((rc = open_destination(ctx, grid, pl)) != GPR_OK) return rc;
+  if ((rc = open_destination(ctx, grid, plane, &a.g, &a.plane)) != GPR_OK) return rc;
   CU(cudaMemsetAsync(ctx->d_sstats, 0, 2 * sizeof(unsigned long long), ctx->stream));
-  a.n_series = S, a.plane = pl, a.stats = ctx->d_sstats;
-  if (total && batch->mem_kind == GPR_MEM_DEVICE) {  // read in place
+  a.n_series = S, a.stats = ctx->d_sstats;
+  if (total && !host) {  // read in place
     a.offsets = batch->offsets, a.rows = batch->rows, a.ts = batch->ts_ms, a.values = batch->values;
     a.base = 0, a.end = total, a.s_base = 0;
     rc = launch_scatter(ctx, a, aligned16(batch->ts_ms) && aligned16(batch->values));
   } else if (total) {
     rc = scatter_host_pieces(ctx, batch, total, a);
   }
-  if (rc != GPR_OK) {
-    (void)cudaStreamSynchronize(ctx->stream);  // the staging buffers may still be read
-    return rc;
-  }
-  unsigned long long counts[2] = {0, 0};
-  CU(cudaMemcpyAsync(counts, ctx->d_sstats, sizeof counts, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaStreamSynchronize(ctx->stream));
-  if (stats) stats->n_in = total, stats->n_oow = counts[0], stats->n_tiny = counts[1];
-  return GPR_OK;
+  return finish_merge(ctx, rc, total, stats);
   GPR_CATCH(ctx)
 }
 
@@ -2169,24 +2163,14 @@ static int chunk_batch_fault(gpr_ctx* ctx, uint32_t bad, uint64_t first, uint32_
 }
 
 static int launch_chunks_check(gpr_ctx* ctx, const gpr::chunks::CheckArgs& a) {
-  const uint32_t blocks = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((a.end - a.base + 255) / 256,
-                                                                            (uint64_t)ctx->sm_count * 8));
-  gpr::chunks::k_chunks_check<<<blocks, 256, 0, ctx->stream>>>(a);
-  ctx->launches++;
-  CU(cudaGetLastError());
-  return GPR_OK;
+  return launch(ctx, gpr::chunks::k_chunks_check, capped_grid(ctx, a.end - a.base, 256, 8), 256, 0, false, a);
 }
 
 static int launch_chunks_scatter(gpr_ctx* ctx, const gpr::chunks::ScatterArgs& a) {
   namespace gc = gpr::chunks;
   if (a.end <= a.base) return GPR_OK;
   const uint64_t groups = (a.end - a.base + 31) / 32;
-  const uint32_t blocks = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((groups + gc::kWarps - 1) / gc::kWarps,
-                                                                            (uint64_t)ctx->sm_count * 8));
-  gc::k_chunks_scatter<<<blocks, gc::kThreads, 0, ctx->stream>>>(a);
-  ctx->launches++;
-  CU(cudaGetLastError());
-  return GPR_OK;
+  return launch(ctx, gc::k_chunks_scatter, capped_grid(ctx, groups, gc::kWarps, 8), gc::kThreads, 0, false, a);
 }
 
 // A host batch's chunk data, piece by piece: each piece is the most whole chunks that fit kHostPiece bytes, and at
@@ -2218,30 +2202,19 @@ int gpr_chunks_scatter(gpr_ctx* ctx, const gpr_chunk_batch* batch, const gpr_tex
   NvtxRange nvtx_range("gpr_chunks_scatter");
   namespace gc = gpr::chunks;
   namespace gs = gpr::samples;
-  if (!batch || batch->struct_size != sizeof(gpr_chunk_batch))
-    return fail(ctx, GPR_E_INVALID, "batch is NULL / struct_size mismatch");
-  if (!grid || grid->struct_size != sizeof(gpr_text_grid)) return fail(ctx, GPR_E_INVALID, "grid is NULL / struct_size mismatch");
-  if (plane < 0 || plane > 1) return fail(ctx, GPR_E_INVALID, "bad plane %d", plane);
-  if (batch->mem_kind != GPR_MEM_HOST && batch->mem_kind != GPR_MEM_DEVICE)
-    return fail(ctx, GPR_E_INVALID, "bad mem_kind %d", batch->mem_kind);
   int rc;
-  if ((rc = check_grid(ctx, grid)) != GPR_OK) return rc;
+  if ((rc = enter(ctx)) != GPR_OK || (rc = check_batch_args(ctx, batch, grid, plane)) != GPR_OK) return rc;
   const uint32_t S = batch->n_series;
+  const bool host = batch->mem_kind == GPR_MEM_HOST;
   if (!batch->series_chunks || !batch->chunk_bytes || (S && !batch->rows))
     return fail(ctx, GPR_E_INVALID, "series_chunks / chunk_bytes / rows is NULL");
-  CU(cudaSetDevice(ctx->device));
-  ctx->last_was_reduce = false;
-  CU(ctx->d_sstats.grow(ctx->stream, 5));  // [n_oow, n_tiny, check word, n_in, first bad chunk]
-  unsigned int* d_bad = reinterpret_cast<unsigned int*>(ctx->d_sstats + 2);
-  const bool host = batch->mem_kind == GPR_MEM_HOST;
   // ---- the batch is checked before anything is written: the index arrays, then the chunks' data
   uint32_t bad = 0;
   uint64_t n_chunks = 0, first = ~0ull;
+  if ((rc = check_series_index(ctx, batch->series_chunks, batch->rows, S, host, grid->n_rows, &bad, &n_chunks)) != GPR_OK)
+    return rc;
+  if (bad) return chunk_batch_fault(ctx, bad, 0, grid->n_rows);
   if (host) {
-    for (uint32_t s = 0; s < std::max(S, 1u); ++s)
-      bad |= gs::series_faults(batch->series_chunks, batch->rows, S, s, grid->n_rows);
-    if (bad) return chunk_batch_fault(ctx, bad, 0, grid->n_rows);
-    n_chunks = batch->series_chunks[S];
     if (batch->chunk_bytes[0] != 0) bad |= gc::kBadChunkStart;
     for (uint64_t c = 0; c < n_chunks && !bad; ++c) {
       bad = gc::bound_faults(batch->chunk_bytes, c);
@@ -2249,33 +2222,18 @@ int gpr_chunks_scatter(gpr_ctx* ctx, const gpr_chunk_batch* batch, const gpr_tex
       if (bad) first = c;
     }
     if (bad) return chunk_batch_fault(ctx, bad, first, grid->n_rows);
-  } else {
-    unsigned long long back[2] = {0, 0};  // the check word, series_chunks[n_series]
-    CU(cudaMemsetAsync(d_bad, 0, sizeof(unsigned long long), ctx->stream));
-    const uint32_t blocks = std::max(1u, std::min((std::max(S, 1u) + 255u) / 256u, (uint32_t)ctx->sm_count * 8u));
-    gs::k_samples_check<<<blocks, 256, 0, ctx->stream>>>(batch->series_chunks, batch->rows, S, grid->n_rows, d_bad);
-    ctx->launches++;
-    CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(&back[0], d_bad, sizeof back[0], cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaMemcpyAsync(&back[1], batch->series_chunks + S, sizeof back[1], cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
-    bad = (uint32_t)back[0], n_chunks = back[1];
-    if (bad) return chunk_batch_fault(ctx, bad, 0, grid->n_rows);
   }
   if (n_chunks && !batch->data) return fail(ctx, GPR_E_INVALID, "data is NULL");
   // the chunks' data, by the check kernel: in place for a device batch, piece by piece as it lands for a host one
   CU(cudaMemsetAsync(ctx->d_sstats + 2, 0, 2 * sizeof(unsigned long long), ctx->stream));
   CU(cudaMemsetAsync(ctx->d_sstats + 4, 0xFF, sizeof(unsigned long long), ctx->stream));
   gc::CheckArgs ck;
-  ck.bad = d_bad, ck.n_in = ctx->d_sstats + 3, ck.first = ctx->d_sstats + 4;
+  ck.bad = reinterpret_cast<unsigned int*>(ctx->d_sstats + 2), ck.n_in = ctx->d_sstats + 3, ck.first = ctx->d_sstats + 4;
   const bool pinned = host && host_pinned(batch->data, nullptr);
   std::vector<gs::Piece> checked;  // a host batch's pieces, in the order they went up
   if (host) {
-    CU(ctx->d_soffsets.grow(ctx->stream, (size_t)S + 1));
-    CU(ctx->d_srows.grow(ctx->stream, (size_t)S + 1));
+    if ((rc = upload_series_index(ctx, batch->series_chunks, batch->rows, S)) != GPR_OK) return rc;
     CU(ctx->d_cbytes.grow(ctx->stream, (size_t)n_chunks + 1));
-    CU(cudaMemcpyAsync(ctx->d_soffsets, batch->series_chunks, ((size_t)S + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
-    CU(cudaMemcpyAsync(ctx->d_srows, batch->rows, (size_t)S * 4, cudaMemcpyHostToDevice, ctx->stream));
     CU(cudaMemcpyAsync(ctx->d_cbytes, batch->chunk_bytes, ((size_t)n_chunks + 1) * 8, cudaMemcpyHostToDevice,
                        ctx->stream));
     if ((rc = open_staging(ctx, pinned)) != GPR_OK) return rc;
@@ -2289,22 +2247,17 @@ int gpr_chunks_scatter(gpr_ctx* ctx, const gpr_chunk_batch* batch, const gpr_tex
     ck.chunk_bytes = batch->chunk_bytes, ck.data = batch->data, ck.data_base = 0, ck.base = 0, ck.end = n_chunks;
     rc = launch_chunks_check(ctx, ck);
   }
-  if (rc != GPR_OK) {
-    (void)cudaStreamSynchronize(ctx->stream);  // the staging buffers may still be read
-    return rc;
-  }
+  if ((rc = drain_on_error(ctx, rc)) != GPR_OK) return rc;
   unsigned long long back[3] = {0, 0, 0};  // the check word, n_in, the first bad chunk
   CU(cudaMemcpyAsync(back, ctx->d_sstats + 2, sizeof back, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   if (back[0]) return chunk_batch_fault(ctx, (uint32_t)back[0], back[2], grid->n_rows);
   // ---- the destination, then the merge
-  float* pl = nullptr;
   gc::ScatterArgs a;
   memset(&a, 0, sizeof a);
-  if ((rc = text_destination(ctx, grid, plane, &a.g, &pl)) != GPR_OK) return rc;
-  if ((rc = open_destination(ctx, grid, pl)) != GPR_OK) return rc;
+  if ((rc = open_destination(ctx, grid, plane, &a.g, &a.plane)) != GPR_OK) return rc;
   CU(cudaMemsetAsync(ctx->d_sstats, 0, 2 * sizeof(unsigned long long), ctx->stream));
-  a.n_series = S, a.plane = pl, a.stats = ctx->d_sstats;
+  a.n_series = S, a.stats = ctx->d_sstats;
   if (!host) {  // read in place
     a.series_chunks = batch->series_chunks, a.rows = batch->rows, a.chunk_bytes = batch->chunk_bytes;
     a.data = batch->data, a.data_base = 0, a.base = 0, a.end = n_chunks, a.s_base = 0;
@@ -2322,26 +2275,12 @@ int gpr_chunks_scatter(gpr_ctx* ctx, const gpr_chunk_batch* batch, const gpr_tex
       rc = chunk_pieces(ctx, batch, n_chunks, pinned, scatter);
     }
   }
-  if (rc != GPR_OK) {
-    (void)cudaStreamSynchronize(ctx->stream);  // the staging buffers may still be read
-    return rc;
-  }
-  unsigned long long counts[2] = {0, 0};
-  CU(cudaMemcpyAsync(counts, ctx->d_sstats, sizeof counts, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaStreamSynchronize(ctx->stream));
-  if (stats) stats->n_in = back[1], stats->n_oow = counts[0], stats->n_tiny = counts[1];
-  return GPR_OK;
+  return finish_merge(ctx, rc, back[1], stats);
   GPR_CATCH(ctx)
 }
 
 // ---- the resident ring as XOR chunks (gpr_chunks_encode.cuh) --------------------------------------------------
 static_assert(sizeof(gpr_chunk_export) == 96, "gpr_chunk_export");
-
-static uint32_t export_grid(gpr_ctx* ctx, uint32_t rows) {
-  namespace gc = gpr::chunks;
-  return (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)rows + gc::kEncWarps - 1) / gc::kEncWarps,
-                                                            (uint64_t)ctx->sm_count * 16));
-}
 
 int gpr_resident_export(gpr_ctx* ctx, const gpr_text_grid* grid, int32_t plane, uint32_t max_per_chunk,
                         gpr_chunk_export* out) {
@@ -2349,6 +2288,7 @@ int gpr_resident_export(gpr_ctx* ctx, const gpr_text_grid* grid, int32_t plane, 
   GPR_TRY
   NvtxRange nvtx_range("gpr_resident_export");
   namespace gc = gpr::chunks;
+  if (const int rc = enter(ctx)) return rc;
   if (!out || out->struct_size != sizeof(gpr_chunk_export))
     return fail(ctx, GPR_E_INVALID, "out is NULL / struct_size mismatch");
   out->n_series = out->n_chunks = out->n_bytes = out->n_samples = 0;
@@ -2367,8 +2307,6 @@ int gpr_resident_export(gpr_ctx* ctx, const gpr_text_grid* grid, int32_t plane, 
   if ((rc = check_grid(ctx, grid)) != GPR_OK) return rc;
   if (grid->n_samples != ctx->res_T)
     return fail(ctx, GPR_E_INVALID, "grid.n_samples %u is not the resident window's %u", grid->n_samples, ctx->res_T);
-  CU(cudaSetDevice(ctx->device));
-  ctx->last_was_reduce = false;
   const uint32_t rows = ctx->res_P * ctx->res_G, T = ctx->res_T;
   gc::ExportArgs a;
   memset(&a, 0, sizeof a);
@@ -2384,11 +2322,10 @@ int gpr_resident_export(gpr_ctx* ctx, const gpr_text_grid* grid, int32_t plane, 
   a.sizes = ctx->d_xsizes, a.row_chunks = ctx->d_xrows, a.row_bytes = ctx->d_xrows + rows + 1;
   a.row_series = ctx->d_xseries, a.totals = ctx->d_xtotals;
   CU(cudaMemsetAsync(a.totals, 0, 4 * sizeof(unsigned long long), ctx->stream));
-  const uint32_t blocks = export_grid(ctx, rows);
-  gc::k_export_size<<<blocks, gc::kEncThreads, 0, ctx->stream>>>(a);
-  gc::k_export_scan<<<1, gc::kScanThreads, gc::kScanSmem, ctx->stream>>>(a);
-  ctx->launches += 2;
-  CU(cudaGetLastError());
+  const uint32_t blocks = capped_grid(ctx, rows, gc::kEncWarps, 16);
+  if ((rc = launch(ctx, gc::k_export_size, blocks, gc::kEncThreads, 0, false, a)) != GPR_OK ||
+      (rc = launch(ctx, gc::k_export_scan, 1, gc::kScanThreads, gc::kScanSmem, false, a)) != GPR_OK)
+    return rc;
   unsigned long long tot[4];
   CU(cudaMemcpyAsync(tot, a.totals, sizeof tot, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
@@ -2408,9 +2345,7 @@ int gpr_resident_export(gpr_ctx* ctx, const gpr_text_grid* grid, int32_t plane, 
   } else {
     a.series_chunks = out->series_chunks, a.out_rows = out->rows, a.chunk_bytes = out->chunk_bytes, a.data = out->data;
   }
-  gc::k_export_write<<<blocks, gc::kEncThreads, 0, ctx->stream>>>(a);
-  ctx->launches++;
-  CU(cudaGetLastError());
+  if ((rc = launch(ctx, gc::k_export_write, blocks, gc::kEncThreads, 0, false, a)) != GPR_OK) return rc;
   if (host) {
     CU(cudaMemcpyAsync(out->series_chunks, a.series_chunks, b_sc, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaMemcpyAsync(out->chunk_bytes, a.chunk_bytes, b_cb, cudaMemcpyDeviceToHost, ctx->stream));
@@ -2425,18 +2360,16 @@ int gpr_resident_export(gpr_ctx* ctx, const gpr_text_grid* grid, int32_t plane, 
 int gpr_synth_fill(gpr_ctx* ctx, uint64_t seed, int32_t plane, float* dst, uint64_t pod_offset,
                    uint32_t n_pods, uint32_t n_gpus, uint32_t n_samples, uint64_t row_stride) {
   if (!ctx) return GPR_E_INVALID;
+  if (const int rc = enter(ctx)) return rc;
   if (!dst || n_gpus == 0 || n_samples == 0 || (plane != 0 && plane != 1))
     return fail(ctx, GPR_E_INVALID, "bad gpr_synth_fill arguments");
   const uint64_t rows = (uint64_t)n_pods * n_gpus;
   if (rows == 0) return GPR_OK;
-  ctx->last_was_reduce = false;
   if (rows > 0x7fffffffull) return fail(ctx, GPR_E_INVALID, "too many series");
-  CU(cudaSetDevice(ctx->device));
   const uint64_t ld = row_stride ? row_stride : n_samples;
-  const uint32_t grid = (uint32_t)std::min<uint64_t>(rows, (uint64_t)ctx->sm_count * 32);
-  gpr::k_synth_fill<<<grid, 256, 0, ctx->stream>>>(dst, seed, plane, pod_offset * n_gpus,
-                                                   (uint32_t)rows, n_samples, ld);
-  CU(cudaGetLastError());
+  if (const int rc = launch(ctx, gpr::k_synth_fill, capped_grid(ctx, rows, 1, 32), 256, 0, false, dst, seed, plane,
+                            pod_offset * n_gpus, (uint32_t)rows, n_samples, ld))
+    return rc;
   CU(cudaStreamSynchronize(ctx->stream));
   return GPR_OK;
 }
@@ -2444,13 +2377,12 @@ int gpr_synth_fill(gpr_ctx* ctx, uint64_t seed, int32_t plane, float* dst, uint6
 int gpr_synth_eligible(gpr_ctx* ctx, uint64_t seed, uint8_t* dst, uint64_t pod_offset,
                        uint32_t n_pods) {
   if (!ctx) return GPR_E_INVALID;
+  if (const int rc = enter(ctx)) return rc;
   if (!dst) return fail(ctx, GPR_E_INVALID, "dst is NULL");
   if (n_pods == 0) return GPR_OK;
-  ctx->last_was_reduce = false;
-  CU(cudaSetDevice(ctx->device));
-  const uint32_t grid = std::min<uint32_t>((n_pods + 255u) / 256u, (uint32_t)ctx->sm_count * 8u);
-  gpr::k_synth_eligible<<<grid, 256, 0, ctx->stream>>>(dst, seed, pod_offset, n_pods);
-  CU(cudaGetLastError());
+  if (const int rc = launch(ctx, gpr::k_synth_eligible, capped_grid(ctx, n_pods, 256, 8), 256, 0, false, dst, seed,
+                            pod_offset, n_pods))
+    return rc;
   CU(cudaStreamSynchronize(ctx->stream));
   return GPR_OK;
 }
@@ -2460,7 +2392,7 @@ int gpr_synth_eligible(gpr_ctx* ctx, uint64_t seed, uint8_t* dst, uint64_t pod_o
 #ifdef GPR_TIMELINE
 extern "C" GPR_API int gpr_debug_timeline(gpr_ctx* ctx, unsigned long long* out, int n_ctas) {
   if (!ctx || !out) return GPR_E_INVALID;
-  CU(cudaSetDevice(ctx->device));
+  if (const int rc = enter(ctx)) return rc;
   CU(cudaStreamSynchronize(ctx->stream));
   CU(cudaMemcpyFromSymbol(out, gpr::g_timeline, sizeof(unsigned long long) * 4 * (size_t)n_ctas));
   return GPR_OK;

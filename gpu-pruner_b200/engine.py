@@ -80,6 +80,28 @@ def _ptr(x) -> Optional[int]:
     raise TypeError(f"cannot take the address of {type(x)!r}")
 
 
+def _n_series(n_series: Optional[int], rows, mem_kind: int) -> int:
+    """a batch's series count: as given, or for host arrays the length of ``rows``"""
+    if n_series is not None:
+        return int(n_series)
+    if mem_kind != ffi.GPR_MEM_HOST:
+        raise ValueError("n_series is required for device arrays")
+    return rows.size
+
+
+def _text_grid(t_end: int, step: int, T: int, n_rows: int = 0, window_seconds: Optional[int] = None,
+               power_threshold: Optional[float] = 0.0, fill: bool = False, resident: bool = False) -> ffi.gpr_text_grid:
+    """the time axis and destination of a merge or an export; ``window_seconds`` defaults to ``T * step``"""
+    g = ffi.gpr_text_grid()
+    g.struct_size = C.sizeof(ffi.gpr_text_grid)
+    g.flags = (ffi.GPR_TEXT_FILL if fill and not resident else 0) | (ffi.GPR_TEXT_RESIDENT if resident else 0)
+    g.t_end, g.step = int(t_end), int(step)
+    g.window_seconds = int(T) * int(step) if window_seconds is None else int(window_seconds)
+    g.n_samples, g.n_rows = int(T), int(n_rows)
+    g.power_threshold = 0.0 if power_threshold is None else float(power_threshold)
+    return g
+
+
 class IdleEngine:
     """One context = one GPU.  Not re-entrant (one call at a time), thread-agnostic."""
 
@@ -425,13 +447,7 @@ class IdleEngine:
         their out-fields filled.  ``window_seconds`` defaults to ``T * step``.  ``power_threshold``: for the
         power plane, the threshold it will be decided with (samples are snapped to it, include/gpr.h)."""
         spans = np.ascontiguousarray(spans, dtype=self.SPAN_DTYPE)
-        g = ffi.gpr_text_grid()
-        g.struct_size = C.sizeof(ffi.gpr_text_grid)
-        g.flags = (ffi.GPR_TEXT_FILL if fill and not resident else 0) | (ffi.GPR_TEXT_RESIDENT if resident else 0)
-        g.t_end, g.step = int(t_end), int(step)
-        g.window_seconds = int(T) * int(step) if window_seconds is None else int(window_seconds)
-        g.n_samples, g.n_rows = int(T), int(n_rows)
-        g.power_threshold = 0.0 if power_threshold is None else float(power_threshold)
+        g = _text_grid(t_end, step, T, n_rows, window_seconds, power_threshold, fill, resident)
         self._check(self._lib.gpr_text_parse(self._h, slot, _ptr(spans), len(spans), C.byref(g), plane))
         return spans
 
@@ -450,22 +466,13 @@ class IdleEngine:
             rows = np.ascontiguousarray(rows, dtype=np.uint32)
             ts_ms = np.ascontiguousarray(ts_ms, dtype=np.int64)
             values = np.ascontiguousarray(values, dtype=np.float64)
-            if n_series is None:
-                n_series = rows.size
-        elif n_series is None:
-            raise ValueError("n_series is required for device arrays")
+        n_series = _n_series(n_series, rows, mem_kind)
         b = ffi.gpr_sample_batch()
         b.struct_size = C.sizeof(ffi.gpr_sample_batch)
         b.mem_kind = mem_kind
         b.offsets, b.rows, b.ts_ms, b.values = _ptr(offsets), _ptr(rows), _ptr(ts_ms), _ptr(values)
-        b.n_series = int(n_series)
-        g = ffi.gpr_text_grid()
-        g.struct_size = C.sizeof(ffi.gpr_text_grid)
-        g.flags = (ffi.GPR_TEXT_FILL if fill and not resident else 0) | (ffi.GPR_TEXT_RESIDENT if resident else 0)
-        g.t_end, g.step = int(t_end), int(step)
-        g.window_seconds = int(T) * int(step) if window_seconds is None else int(window_seconds)
-        g.n_samples, g.n_rows = int(T), int(n_rows)
-        g.power_threshold = 0.0 if power_threshold is None else float(power_threshold)
+        b.n_series = n_series
+        g = _text_grid(t_end, step, T, n_rows, window_seconds, power_threshold, fill, resident)
         st = ffi.gpr_sample_stats()
         self._check(self._lib.gpr_samples_scatter(self._h, C.byref(b), C.byref(g), plane, C.byref(st)))
         return {"n_in": st.n_in, "n_oow": st.n_oow, "n_tiny": st.n_tiny}
@@ -486,22 +493,13 @@ class IdleEngine:
             chunk_bytes = np.ascontiguousarray(chunk_bytes, dtype=np.uint64)
             data = np.ascontiguousarray(np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray))
                                         else data, dtype=np.uint8)
-            if n_series is None:
-                n_series = rows.size
-        elif n_series is None:
-            raise ValueError("n_series is required for device arrays")
+        n_series = _n_series(n_series, rows, mem_kind)
         b = ffi.gpr_chunk_batch()
         b.struct_size = C.sizeof(ffi.gpr_chunk_batch)
         b.mem_kind = mem_kind
         b.series_chunks, b.rows, b.chunk_bytes, b.data = _ptr(series_chunks), _ptr(rows), _ptr(chunk_bytes), _ptr(data)
-        b.n_series = int(n_series)
-        g = ffi.gpr_text_grid()
-        g.struct_size = C.sizeof(ffi.gpr_text_grid)
-        g.flags = (ffi.GPR_TEXT_FILL if fill and not resident else 0) | (ffi.GPR_TEXT_RESIDENT if resident else 0)
-        g.t_end, g.step = int(t_end), int(step)
-        g.window_seconds = int(T) * int(step) if window_seconds is None else int(window_seconds)
-        g.n_samples, g.n_rows = int(T), int(n_rows)
-        g.power_threshold = 0.0 if power_threshold is None else float(power_threshold)
+        b.n_series = n_series
+        g = _text_grid(t_end, step, T, n_rows, window_seconds, power_threshold, fill, resident)
         st = ffi.gpr_sample_stats()
         self._check(self._lib.gpr_chunks_scatter(self._h, C.byref(b), C.byref(g), plane, C.byref(st)))
         return {"n_in": st.n_in, "n_oow": st.n_oow, "n_tiny": st.n_tiny}
@@ -514,12 +512,7 @@ class IdleEngine:
         (``series_chunks``, ``rows``, ``chunk_bytes``, ``data``), the counts ``n_samples``, and the ``grid`` to
         restore with: ``chunks_scatter(..., **out["grid"], resident=True)`` into a ring of the same T."""
         T = int(self.resident_planes()[2])
-        g = ffi.gpr_text_grid()
-        g.struct_size = C.sizeof(ffi.gpr_text_grid)
-        g.t_end, g.step = int(t_end), int(step)
-        g.window_seconds = T * int(step) if window_seconds is None else int(window_seconds)
-        g.n_samples = T
-        g.power_threshold = 0.0 if power_threshold is None else float(power_threshold)
+        g = _text_grid(t_end, step, T, window_seconds=window_seconds, power_threshold=power_threshold)
         o = ffi.gpr_chunk_export()
         o.struct_size = C.sizeof(ffi.gpr_chunk_export)
         o.mem_kind = ffi.GPR_MEM_HOST
