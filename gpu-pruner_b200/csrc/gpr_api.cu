@@ -445,14 +445,14 @@ int launch_reduce(gpr_ctx* ctx, gpr::ReduceParams& rp, bool tma_ok, bool pdl) {
   return rp.grouped ? launch_reduce_as<true>(ctx, rp, tma_ok, pdl) : launch_reduce_as<false>(ctx, rp, tma_ok, pdl);
 }
 
-int copy_rows_h2d(gpr_ctx* ctx, void* dst, const void* src, size_t n_rows, uint32_t T,
-                  uint64_t ld, size_t esize, cudaStream_t s) {
+// n_rows rows of T elements, `ld` elements apart in src, to dense rows at dst: one plain copy when src is dense too
+int copy_rows(gpr_ctx* ctx, void* dst, const void* src, size_t n_rows, uint64_t T, uint64_t ld, size_t esize,
+              cudaMemcpyKind kind, cudaStream_t s) {
   if (n_rows == 0) return GPR_OK;
   if (ld == T) {
-    CU(cudaMemcpyAsync(dst, src, n_rows * (size_t)T * esize, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dst, src, n_rows * (size_t)T * esize, kind, s));
   } else {
-    CU(cudaMemcpy2DAsync(dst, (size_t)T * esize, src, (size_t)ld * esize, (size_t)T * esize, n_rows,
-                         cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpy2DAsync(dst, (size_t)T * esize, src, (size_t)ld * esize, (size_t)T * esize, n_rows, kind, s));
   }
   return GPR_OK;
 }
@@ -462,9 +462,26 @@ struct NvtxRange {
   ~NvtxRange() { nvtxRangePop(); }
 };
 
-int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resident, bool async) {
-  if (!ctx) return GPR_E_INVALID;
-  NvtxRange nvtx_range(resident ? "gpr_decide_resident" : "gpr_decide");
+// What a decision reads (the caller's window, or the resident ring or its block index) and its shape, as read_window
+// resolved and checked it
+struct Window {
+  uint32_t P, G, T;
+  uint32_t MW, W, S;        // mask words per pod, bitmap words, series
+  uint64_t ld;              // elements between rows
+  const float* util;        // biased bytes when u8
+  const float* power;
+  const uint32_t* groups;   // nullptr for a caller built before gpr_window.groups existed
+  uint32_t* idle_slots;     // nullptr for a caller built before gpr_result.idle_slots existed
+  bool u8, use_power;
+  bool host_in;             // util and power are in host memory and go up in pieces through the staging planes
+  bool host_arrays;         // the gates and the group table are in host memory (mem_kind, for the ring too)
+  bool grouped;             // a group table over one pod or more
+  bool fused, comm;         // the bitmaps are exchanged between ranks (fused: over peer memory, else by NCCL)
+};
+
+// Every check of a decision, before anything is enqueued: the structs, the window, the result, the exchange, the host
+// group table and the staging capacity.
+int read_window(gpr_ctx* ctx, const gpr_window* win, const gpr_result* res, bool resident, Window* w) {
   if (!win || !res) return fail(ctx, GPR_E_INVALID, "window/result is NULL");
   // a caller built before gpr_window.groups / gpr_result.idle_slots existed passes the older sizes: no such fields
   const size_t win_v1 = offsetof(gpr_window, groups), res_v1 = offsetof(gpr_result, idle_slots);
@@ -516,8 +533,6 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
   const uint32_t W = (P + 31u) / 32u;
   const bool use_power = power != nullptr && power_truthy(win->power_threshold);
   const bool host_in = !resident && in_kind == GPR_MEM_HOST;
-  const bool gates_host = in_kind == GPR_MEM_HOST;
-  const bool host_out = res->out_mem_kind == GPR_MEM_HOST;
   const bool fused = ctx->p2p_ready && ctx->world > 1;
   const bool comm = (ctx->comm != nullptr || fused) && ctx->world > 1;
   if (fused && 2u * W > ctx->p2p_stride)
@@ -550,9 +565,24 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
     if (use_power && !ctx->cap_power)
       return fail(ctx, GPR_E_CAPACITY, "power plane not reserved (GPR_F_POWER_PLANE)");
   }
+  w->P = P, w->G = G, w->T = T, w->MW = MW, w->W = W, w->S = S, w->ld = ld;
+  w->util = util, w->power = power, w->groups = groups, w->idle_slots = idle_slots;
+  w->u8 = u8, w->use_power = use_power, w->host_in = host_in, w->host_arrays = in_kind == GPR_MEM_HOST;
+  w->grouped = grouped, w->fused = fused, w->comm = comm;
+  return GPR_OK;
+}
+
+int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resident, bool async) {
+  NvtxRange nvtx_range(resident ? "gpr_decide_resident" : "gpr_decide");
+  Window w{};
+  int rc = read_window(ctx, win, res, resident, &w);
+  if (rc != GPR_OK) return rc;
+  const uint32_t P = w.P, G = w.G, T = w.T, MW = w.MW, W = w.W, S = w.S;
+  const bool use_power = w.use_power, host_in = w.host_in, grouped = w.grouped, fused = w.fused;
+  const bool nccl = w.comm && !w.fused;  // the bitmaps are gathered by ncclAllGather after the fold
+  const bool host_out = res->out_mem_kind == GPR_MEM_HOST;
 
   // ---- scratch ---------------------------------------------------------------------------
-  int rc;
   const unsigned sset = ctx->parity;  // scratch set of this call; successive calls alternate
   ctx->parity ^= 1u;
   if (ctx->masks_dirty) {  // a failed launch may also have left ticket / accumulators behind
@@ -571,21 +601,21 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
   ctx->masks_dirty = false;
   uint32_t* const masks = ctx->d_masks[sset];
   CU(ctx->d_bits.grow(ctx->stream, (size_t)3 * W + 2));
-  if (comm && !fused) CU(ctx->d_gather.grow(ctx->stream, (size_t)ctx->world * 2 * W + 2));
+  if (nccl) CU(ctx->d_gather.grow(ctx->stream, (size_t)ctx->world * 2 * W + 2));
   const bool want_smax = res->series_max != nullptr;
   if (want_smax && host_out) CU(ctx->d_smax.grow(ctx->stream, (size_t)S + 4));
-  if (idle_slots && host_out) CU(ctx->d_islots.grow(ctx->stream, (size_t)P * MW + 4));
+  if (w.idle_slots && host_out) CU(ctx->d_islots.grow(ctx->stream, (size_t)P * MW + 4));
   if (grouped) {
     CU(ctx->d_grouped.grow(ctx->stream, (size_t)P * MW + 4));
     CU(ctx->d_gpods.grow(ctx->stream, (size_t)P + 4));
     if (!want_smax) CU(ctx->d_gmax.grow(ctx->stream, (size_t)S + 4));
-    if (in_kind == GPR_MEM_HOST) CU(ctx->d_gtable.grow(ctx->stream, (size_t)S + 4));
+    if (w.host_arrays) CU(ctx->d_gtable.grow(ctx->stream, (size_t)S + 4));
   }
 
   // ---- gates -----------------------------------------------------------------------------
   const uint8_t* d_elig = win->eligible;
   const int64_t* d_created = win->created_ts;
-  if (gates_host && (win->eligible || win->created_ts)) {
+  if (w.host_arrays && (win->eligible || win->created_ts)) {
     CU(ctx->d_elig_stage.grow(ctx->stream, P));
     CU(ctx->d_created_stage.grow(ctx->stream, P));
     ctx->last_was_reduce = false;
@@ -601,10 +631,10 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
   }
 
   // ---- output targets --------------------------------------------------------------------
-  const bool direct_bits = !host_out && !comm;
+  const bool direct_bits = !host_out && !w.comm;
   uint32_t* dbits_dev = direct_bits ? res->decision_bits : ctx->d_bits;
   uint32_t* cbits_dev = direct_bits ? res->candidate_bits
-                                    : ((res->candidate_bits || comm) ? ctx->d_bits + W : nullptr);
+                                    : ((res->candidate_bits || w.comm) ? ctx->d_bits + W : nullptr);
   // pods vetoed by the power clause: never exchanged (this rank's pods only)
   uint32_t* vbits_dev = res->veto_bits ? (host_out ? ctx->d_bits + 2 * (size_t)W : res->veto_bits) : nullptr;
   uint32_t* my_gather = nullptr;  // local gather buffer of this call (fused exchange)
@@ -617,9 +647,9 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
   // (a series_max target also tells the reduce kernels to read every row whole: the true max is an output; without
   // one they stop reading a row at the first sample that settles its flag, gpr_kernels.cuh "early exit")
   float* smax_dev = want_smax ? (host_out ? ctx->d_smax : res->series_max) : nullptr;
-  uint32_t* islots_dev = idle_slots ? (host_out ? ctx->d_islots : idle_slots) : nullptr;
+  uint32_t* islots_dev = w.idle_slots ? (host_out ? ctx->d_islots : w.idle_slots) : nullptr;
 
-  gpr::FoldParams fp;
+  gpr::FoldParams fp{};
   fp.idle_mask = masks;
   fp.veto_mask = use_power ? masks + (size_t)P * MW : nullptr;
   fp.eligible = d_elig;
@@ -644,13 +674,9 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
   fp.P = P;
   fp.G = G;
   fp.mw = MW;
-  fp.world = 1, fp.rank = 0;
-  fp.exchange_debug = 0;
+  fp.world = 1;
   fp.poll_ns = ctx->poll_ns;
-  fp.my_ll = nullptr;
-  fp.late_order = 0;
   fp.islots = islots_dev;
-  for (int r = 0; r < gpr::kMaxPeers; ++r) fp.peer_ll[r] = nullptr;
   if (fused) {
     fp.exchange_debug = ctx->exchange_debug;
     fp.world = ctx->world, fp.rank = ctx->rank;
@@ -673,14 +699,15 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
     fp.out_cbits = host_out ? nullptr : res->candidate_bits;
   }
 
-  gpr::ReduceParams rp;
-  memset(&rp, 0, sizeof rp);
+  gpr::ReduceParams rp{};
+  rp.ld = host_in ? T : w.ld;  // staging is dense
   rp.T = T;
   rp.G = G;
   rp.mw = MW;
   rp.thr = threshold_f32(win->power_threshold);
   rp.done = fp.done;
   rp.need = fp.need;
+  rp.util_u8 = w.u8 ? 1u : 0u;
   const bool can_pdl = ctx->pdl_enabled && ctx->own_stream;
   // the fold grid: 32 bitmap words per CTA and round; a handful of CTAs even at millions of pods
   // one bitmap word per warp and round, 4 words per warp in flight (fold_words<4>): small CTAs spread the fold's
@@ -689,12 +716,11 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
   const uint32_t fold_grid = gpr::fold_grid(launch_knobs(ctx), P);
 
   // ---- `sum by` groups: the table's kernels around the reduce (gpr_groups.cuh) -----------------
-  gpr::GroupParams gq;
-  memset(&gq, 0, sizeof gq);
+  gpr::GroupParams gq{};
   if (grouped) {
-    gq.table = groups;
-    if (in_kind == GPR_MEM_HOST) {
-      CU(cudaMemcpyAsync(ctx->d_gtable, groups, (size_t)S * 4u, cudaMemcpyHostToDevice, ctx->stream));
+    gq.table = w.groups;
+    if (w.host_arrays) {
+      CU(cudaMemcpyAsync(ctx->d_gtable, w.groups, (size_t)S * 4u, cudaMemcpyHostToDevice, ctx->stream));
       gq.table = ctx->d_gtable;
     }
     gq.need = ctx->d_grouped;
@@ -704,144 +730,126 @@ int decide_impl(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resid
     gq.idle_mask = masks;
     gq.bad = ctx->h_gerr;
     gq.P = P, gq.G = G, gq.mw = MW;
-    rp.grouped = ctx->d_grouped;
-    rp.gmax = ctx->d_gmax;
     ctx->last_was_reduce = false;   // the group scratch is single-buffered: no PDL into or out of this decision
   }
   const uint32_t group_grid = gpr::group_grid(launch_knobs(ctx), P);
-  auto launch_group_rows = [&]() -> int {
-    CU(cudaMemsetAsync(ctx->d_gpods, 0, sizeof(uint32_t), ctx->stream));
-    return launch(ctx, gpr::k_group_rows, group_grid, gpr::kGroupBlock, 0, false, gq);
-  };
-  auto launch_group_sum = [&]() -> int {
-    return launch(ctx, gpr::k_group_sum, group_grid, gpr::kGroupBlock, 0, false, gq);
-  };
-  const bool fold_pdl = can_pdl && !grouped;
-  auto launch_fold = [&](bool pdl) -> int {
-    const auto k = fused ? (islots_dev ? gpr::k_fold<true, true> : gpr::k_fold<true, false>)
-                         : (islots_dev ? gpr::k_fold<false, true> : gpr::k_fold<false, false>);
-    return launch(ctx, k, fold_grid, fold_threads, 0, pdl, fp);
-  };
 
   if (!async) {
     CU(cudaEventRecord(ctx->ev_k0, ctx->stream));
     ctx->last_was_reduce = false;
   }
 
-  if (!host_in) {
-    // ---- device-resident window: one reduce launch + the PDL-chained fold -------------------
-    rp.ld = ld;
-    rp.seg[0] = gpr::Segment{util, masks, smax_dev, S, 0u};
-    rp.seg[1] = gpr::Segment{power, masks + (size_t)P * MW, nullptr, use_power ? S : 0u, 1u};
-    rp.total_rows = S + (use_power ? S : 0u);
-    rp.util_u8 = u8 ? 1u : 0u;
-    const bool tma_ok = (T % 4u) == 0 && (ld % 4u) == 0 && aligned16(util) &&
-                        (!use_power || aligned16(power));
-    if (P > 0) {
-      // The reduce grid may start while the previous decision's fold is still running, but only
-      // when that is provably safe: our own stream (no foreign producer kernels between), the
-      // newest op on it is one of our fold kernels, and this launch writes nothing but its own
-      // scratch set (series_max would go straight to the caller's buffer).
-      // (nor with a group table: k_group_rows writes the table's single-buffered scratch)
-      const bool pdl = can_pdl && ctx->last_was_reduce && !want_smax && !grouped;
-      if (grouped && (rc = launch_group_rows()) != GPR_OK) return rc;
-      if ((rc = launch_reduce(ctx, rp, tma_ok, pdl)) != GPR_OK) return rc;
-      if (grouped && (rc = launch_group_sum()) != GPR_OK) return rc;
-      if ((rc = launch_fold(fold_pdl)) != GPR_OK) return rc;
-      ctx->uses[sset]++;
-      ctx->last_was_reduce = !grouped;
-    }
-  } else {
-    // ---- host window: pod chunks, H2D on the copy stream overlapped with the reduce --------
+  // ---- the reduce over the window's pieces of whole pods, then the fold --------------------------
+  // A device window is one piece, read in place.  A host window is cut into pieces of chunk_bytes: each is copied
+  // into the dense staging planes on the copy stream, and its reduce waits for that copy only, so the next piece's
+  // copy overlaps it.
+  if (host_in) {
     ctx->last_was_reduce = false;
     CU(cudaEventRecord(ctx->ev_join, ctx->stream));
     CU(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_join, 0));
-    const size_t usize = u8 ? 1u : 4u;  // bytes per util sample on the wire and in the staging plane
+  }
+  if (P > 0) {
+    // The reduce grid may start while the previous decision's fold is still running, but only
+    // when that is provably safe: our own stream (no foreign producer kernels between), the
+    // newest op on it is one of our fold kernels, and this launch writes nothing but its own
+    // scratch set (series_max would go straight to the caller's buffer).
+    // (nor with a group table: k_group_rows writes the table's single-buffered scratch; nor behind a staging copy)
+    const bool chain = can_pdl && !host_in;
+    const bool reduce_pdl = chain && ctx->last_was_reduce && !want_smax && !grouped;
+    const size_t usize = w.u8 ? 1u : 4u;  // bytes per util sample on the wire and in the staging plane
     const size_t pod_bytes = (size_t)G * T * (usize + (use_power ? 4u : 0u));
-    uint32_t chunk_pods = (uint32_t)std::max<size_t>(1, ctx->chunk_bytes / std::max<size_t>(pod_bytes, 1));
-    uint32_t n_chunks = P ? (P + chunk_pods - 1) / chunk_pods : 0;
-    rp.ld = T;  // staging is dense
-    rp.util_u8 = u8 ? 1u : 0u;
-    const bool tma_ok = (T % 4u) == 0;
-    const char* util_bytes = reinterpret_cast<const char*>(util);
-    char* stage_bytes = reinterpret_cast<char*>(ctx->d_util_stage.p);
-    if (grouped && (rc = launch_group_rows()) != GPR_OK) return rc;
-    for (uint32_t c = 0; c < n_chunks; ++c) {
-      const uint32_t p0 = c * chunk_pods, p1 = std::min(P, p0 + chunk_pods);
+    const uint32_t piece_pods =
+        host_in ? (uint32_t)std::max<size_t>(1, ctx->chunk_bytes / std::max<size_t>(pod_bytes, 1)) : P;
+    const uint32_t n_pieces = (P + piece_pods - 1) / piece_pods;
+    // bulk copies need rows of a multiple of 4 samples at 16-byte aligned addresses (the staging planes are dense)
+    const bool tma_ok = (T % 4u) == 0 &&
+                        (host_in || ((w.ld % 4u) == 0 && aligned16(w.util) && (!use_power || aligned16(w.power))));
+    if (grouped) {
+      CU(cudaMemsetAsync(ctx->d_gpods, 0, sizeof(uint32_t), ctx->stream));
+      if ((rc = launch(ctx, gpr::k_group_rows, group_grid, gpr::kGroupBlock, 0, false, gq)) != GPR_OK) return rc;
+    }
+    for (uint32_t c = 0; c < n_pieces; ++c) {
+      const uint32_t p0 = c * piece_pods, p1 = std::min(P, p0 + piece_pods);
       const size_t row0 = (size_t)p0 * G, n_rows = (size_t)(p1 - p0) * G;
-      float* du = reinterpret_cast<float*>(stage_bytes + row0 * T * usize);
-      if ((rc = copy_rows_h2d(ctx, du, util_bytes + row0 * ld * usize, n_rows, T, ld, usize,
-                              ctx->copy_stream)) != GPR_OK)
-        return rc;
-      float* dp = nullptr;
-      if (use_power) {
-        dp = ctx->d_power_stage + row0 * T;
-        if ((rc = copy_rows_h2d(ctx, dp, power + row0 * ld, n_rows, T, ld, 4u, ctx->copy_stream)) !=
-            GPR_OK)
+      const float* pu = w.util;  // a device window's one piece (row0 = 0)
+      const float* pp = w.power;
+      if (host_in) {
+        float* du = reinterpret_cast<float*>(reinterpret_cast<char*>(ctx->d_util_stage.p) + row0 * T * usize);
+        float* dp = use_power ? ctx->d_power_stage + row0 * T : nullptr;
+        if ((rc = copy_rows(ctx, du, reinterpret_cast<const char*>(w.util) + row0 * w.ld * usize, n_rows, T, w.ld,
+                            usize, cudaMemcpyHostToDevice, ctx->copy_stream)) != GPR_OK)
           return rc;
+        if (use_power && (rc = copy_rows(ctx, dp, w.power + row0 * w.ld, n_rows, T, w.ld, 4u, cudaMemcpyHostToDevice,
+                                         ctx->copy_stream)) != GPR_OK)
+          return rc;
+        cudaEvent_t ev = ctx->ev_chunk[c % kMaxChunkEvents];
+        CU(cudaEventRecord(ev, ctx->copy_stream));
+        CU(cudaStreamWaitEvent(ctx->stream, ev, 0));
+        pu = du, pp = dp;
       }
-      cudaEvent_t ev = ctx->ev_chunk[c % kMaxChunkEvents];
-      CU(cudaEventRecord(ev, ctx->copy_stream));
-      CU(cudaStreamWaitEvent(ctx->stream, ev, 0));
-      rp.seg[0] = gpr::Segment{du, masks + (size_t)p0 * MW, smax_dev ? smax_dev + row0 : nullptr,
+      rp.seg[0] = gpr::Segment{pu, masks + (size_t)p0 * MW, smax_dev ? smax_dev + row0 : nullptr,
                                (uint32_t)n_rows, 0u};
-      rp.seg[1] = gpr::Segment{dp, masks + ((size_t)P + p0) * MW, nullptr,
+      rp.seg[1] = gpr::Segment{pp, masks + ((size_t)P + p0) * MW, nullptr,
                                use_power ? (uint32_t)n_rows : 0u, 1u};
       rp.total_rows = (uint32_t)n_rows * (use_power ? 2u : 1u);
       if (grouped) rp.grouped = ctx->d_grouped + (size_t)p0 * MW, rp.gmax = ctx->d_gmax ? ctx->d_gmax + row0 : nullptr;
-      if ((rc = launch_reduce(ctx, rp, tma_ok, false)) != GPR_OK) return rc;
+      if ((rc = launch_reduce(ctx, rp, tma_ok, reduce_pdl)) != GPR_OK) return rc;
     }
-    if (grouped && (rc = launch_group_sum()) != GPR_OK) return rc;
-    if (P > 0) {
-      if ((rc = launch_fold(false)) != GPR_OK) return rc;
-      ctx->uses[sset]++;
-    }
+    if (grouped && (rc = launch(ctx, gpr::k_group_sum, group_grid, gpr::kGroupBlock, 0, false, gq)) != GPR_OK)
+      return rc;
+    const auto fold = fused ? (islots_dev ? gpr::k_fold<true, true> : gpr::k_fold<true, false>)
+                            : (islots_dev ? gpr::k_fold<false, true> : gpr::k_fold<false, false>);
+    if ((rc = launch(ctx, fold, fold_grid, fold_threads, 0, chain && !grouped, fp)) != GPR_OK) return rc;
+    ctx->uses[sset]++;
+    ctx->last_was_reduce = !host_in && !grouped;
   }
   if (P == 0) memset(h_slot, 0, 8 * sizeof(unsigned long long));  // slot is not in flight
 
   // ---- the one collective: allgather of the packed bitmap over NVLink ----------------------
-  if ((comm && !fused) || host_out || !async) ctx->last_was_reduce = false;  // something follows
-  if (comm && !fused && W > 0) {
+  if (nccl || host_out || !async) ctx->last_was_reduce = false;  // something follows
+  if (nccl && W > 0) {
     NC(g_nccl.AllGather(ctx->d_bits, ctx->d_gather, (size_t)2 * W, ncclUint32, ctx->comm,
                         ctx->stream));
   }
   if (!async) CU(cudaEventRecord(ctx->ev_k1, ctx->stream));
 
   // ---- deliver -----------------------------------------------------------------------------
+  // The decision and candidate bitmaps are `rows` rows of W words, `pitch` words apart: this rank's one row in d_bits,
+  // or a row per rank in the fused exchange's gather block or in the NCCL gather buffer.  They are copied for host
+  // outputs, and for device outputs only out of the NCCL buffer (otherwise the fold wrote them in place).  Veto
+  // bits, series_max and idle_slots (this rank's pods) are copied out of their staging for host outputs only.
+  const uint32_t* bits = fused ? my_gather : nccl ? ctx->d_gather : ctx->d_bits;
+  const size_t pitch = fused ? ctx->p2p_stride : nccl ? 2 * (size_t)W : W;
+  const size_t rows = w.comm ? (size_t)ctx->world : 1;
+  const struct {
+    void* dst;
+    const void* src;
+    size_t rows, words, pitch;
+    bool copy;
+  } outs[] = {
+      {res->decision_bits, bits, rows, W, pitch, host_out || nccl},
+      {res->candidate_bits, bits + W, rows, W, pitch, host_out || nccl},
+      {res->veto_bits, ctx->d_bits + 2 * (size_t)W, 1, W, W, host_out},
+      {res->series_max, ctx->d_smax, 1, S, S, host_out},
+      {w.idle_slots, ctx->d_islots, 1, (size_t)P * MW, (size_t)P * MW, host_out},
+  };
   const cudaMemcpyKind out_kind = host_out ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
-  if (W > 0) {
-    if (fused) {
-      if (host_out) {  // device outputs were assembled by the folding CTA itself
-        const size_t pitch = (size_t)ctx->p2p_stride * 4u;
-        CU(cudaMemcpy2DAsync(res->decision_bits, (size_t)W * 4u, my_gather, pitch, (size_t)W * 4u,
-                             ctx->world, out_kind, ctx->stream));
-        if (res->candidate_bits)
-          CU(cudaMemcpy2DAsync(res->candidate_bits, (size_t)W * 4u, my_gather + W, pitch,
-                               (size_t)W * 4u, ctx->world, out_kind, ctx->stream));
-      }
-    } else if (comm) {
-      CU(cudaMemcpy2DAsync(res->decision_bits, (size_t)W * 4u, ctx->d_gather, (size_t)2 * W * 4u,
-                           (size_t)W * 4u, ctx->world, out_kind, ctx->stream));
-      if (res->candidate_bits)
-        CU(cudaMemcpy2DAsync(res->candidate_bits, (size_t)W * 4u, ctx->d_gather + W,
-                             (size_t)2 * W * 4u, (size_t)W * 4u, ctx->world, out_kind, ctx->stream));
-    } else if (host_out) {
-      CU(cudaMemcpyAsync(res->decision_bits, ctx->d_bits, (size_t)W * 4u, out_kind, ctx->stream));
-      if (res->candidate_bits)
-        CU(cudaMemcpyAsync(res->candidate_bits, ctx->d_bits + W, (size_t)W * 4u, out_kind,
-                           ctx->stream));
-    }
-  }
-  if (res->veto_bits && host_out && W > 0)
-    CU(cudaMemcpyAsync(res->veto_bits, ctx->d_bits + 2 * (size_t)W, (size_t)W * 4u, cudaMemcpyDeviceToHost, ctx->stream));
-  if (want_smax && host_out && S > 0)
-    CU(cudaMemcpyAsync(res->series_max, ctx->d_smax, (size_t)S * 4u, cudaMemcpyDeviceToHost,
-                       ctx->stream));
-  if (idle_slots && host_out && P > 0)
-    CU(cudaMemcpyAsync(idle_slots, ctx->d_islots, (size_t)P * MW * 4u, cudaMemcpyDeviceToHost, ctx->stream));
+  for (const auto& o : outs)
+    if (o.copy && o.dst && o.words > 0 &&
+        (rc = copy_rows(ctx, o.dst, o.src, o.rows, o.words, o.pitch, 4u, out_kind, ctx->stream)) != GPR_OK)
+      return rc;
   ctx->pending.push_back(Pending{res, slot});
   res->kernel_ms = 0.0;
   return GPR_OK;
+}
+
+// The one failure rule of a decision: whether a check refused it or a launch or copy failed after part of it was
+// enqueued, the scratch may hold bits, tickets or counts of its own, so the next decision re-zeroes it first.
+int decide(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resident, bool async) {
+  if (!ctx) return GPR_E_INVALID;
+  const int rc = decide_impl(ctx, win, res, resident, async);
+  if (rc != GPR_OK) ctx->masks_dirty = true;
+  return rc;
 }
 
 int sync_impl(gpr_ctx* ctx) {
@@ -1236,9 +1244,7 @@ int gpr_create(const gpr_config* cfg, gpr_ctx** out) {
 
 int gpr_decide_async(gpr_ctx* ctx, const gpr_window* win, gpr_result* res) {
   GPR_TRY
-  const int rc = decide_impl(ctx, win, res, false, true);
-  if (rc != GPR_OK && ctx) ctx->masks_dirty = true;
-  return rc;
+  return decide(ctx, win, res, false, true);
   GPR_CATCH(ctx)
 }
 
@@ -1246,13 +1252,8 @@ int gpr_decide_batch_async(gpr_ctx* ctx, const gpr_window* wins, gpr_result* res
   if (!ctx) return GPR_E_INVALID;
   GPR_TRY
   if (n && (!wins || !results)) return fail(ctx, GPR_E_INVALID, "windows/results is NULL");
-  for (uint32_t i = 0; i < n; ++i) {
-    const int rc = decide_impl(ctx, &wins[i], &results[i], false, true);
-    if (rc != GPR_OK) {
-      ctx->masks_dirty = true;
-      return rc;
-    }
-  }
+  for (uint32_t i = 0; i < n; ++i)
+    if (const int rc = decide(ctx, &wins[i], &results[i], false, true)) return rc;
   return GPR_OK;
   GPR_CATCH(ctx)
 }
@@ -1265,13 +1266,10 @@ int gpr_sync(gpr_ctx* ctx) {
 }
 
 static int decide_blocking(gpr_ctx* ctx, const gpr_window* win, gpr_result* res, bool resident) {
-  int rc = decide_impl(ctx, win, res, resident, false);
-  if (rc != GPR_OK) {
-    // like the async paths: decisions enqueued before this call stay pending, and the next gpr_sync or
-    // successful blocking call fills their counters; this call enqueued no result of its own
-    if (ctx) ctx->masks_dirty = true;
-    return rc;
-  }
+  // like the async paths, a failed call leaves the decisions enqueued before it pending (the next gpr_sync or
+  // successful blocking call fills their counters) and enqueues no result of its own
+  int rc = decide(ctx, win, res, resident, false);
+  if (rc != GPR_OK) return rc;
   rc = sync_impl(ctx);
   if (rc != GPR_OK) return rc;
   float ms = 0.f;
