@@ -13,6 +13,7 @@
 #include "json.hpp"
 #include "kube.hpp"
 #include "promql.hpp"
+#include "snapshot.hpp"
 
 #define GPH_API extern "C" __attribute__((visibility("default")))
 
@@ -77,6 +78,12 @@ GPH_API int gph_render_selectors(const char* args, int n, char* out, int cap) {
   gph::Json j = gph::Json::object();
   j.set("prof", s.prof), j.set("util", s.util), j.set("power", s.power);
   return put(j.dump(), out, cap);
+}
+
+// CRC32C of the snapshot file (snapshot.hpp): portable = 1 forces the slice-by-8 tables, 0 takes the SSE4.2
+// instruction when the CPU has it
+GPH_API unsigned gph_crc32c(const void* data, unsigned long long n, unsigned crc, int portable) {
+  return portable ? gph::crc32c_portable(data, (size_t)n, crc) : gph::crc32c(data, (size_t)n, crc);
 }
 
 GPH_API int gph_enabled_resources(const char* letters) { return gph::get_enabled_resources(letters); }

@@ -42,6 +42,7 @@ std::string usage() {
       "      --patch-out <FILE>                     (extension) write scale-down requests here as JSON lines\n"
       "      --print-query                          (extension) print the rendered PromQL and exit\n"
       "      --gpu-device <N>                       (extension) CUDA device ordinal [default: 0]\n"
+      "      --snapshot-file <PATH>                 (extension) with -d: save the resident window after every tick, resume from it at start\n"
       "  -h, --help                                 Print help\n";
 }
 
@@ -136,6 +137,7 @@ ParseOutcome parse_cli(const std::vector<std::string>& args) {
     if (e.empty()) c.gpu_device = (int)x;
     return e;
   }};
+  specs["snapshot-file"] = {0, true, [&](const std::string& v) { c.snapshot_file = v; return std::string(); }};
   specs["now"] = {0, true, [&](const std::string& v) { return parse_i64(v, &c.now_override); }};
   specs["max-ticks"] = {0, true, [&](const std::string& v) {
     int64_t x;
@@ -198,6 +200,8 @@ ParseOutcome parse_cli(const std::vector<std::string>& args) {
     const std::string err = sp.set(value);
     if (!err.empty()) return fail("invalid value '" + value + "' for '--" + name + "': " + err);
   }
+  if (c.snapshot_file && !c.daemon_mode)
+    return fail("the argument '--snapshot-file <PATH>' can only be used with '--daemon-mode'");
   if (!have_url && !c.print_query)
     return fail("the following required arguments were not provided:\n  --prometheus-url <PROMETHEUS_URL>");
   out.ok = true;

@@ -37,6 +37,8 @@ struct Cli {
   int gpu_device = 0;                         // --gpu-device N
   int64_t now_override = 0;                   // --now UNIX_SECONDS (tests): 0 = wall clock
   int max_ticks = 0;                          // --max-ticks N (tests): stop the daemon loop after N ticks
+  std::optional<std::string> snapshot_file;   // --snapshot-file PATH (-d only): save the resident window after every
+                                              // tick, resume from it at start (DESIGN.md §8i)
 };
 
 struct ParseOutcome {

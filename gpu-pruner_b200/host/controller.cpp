@@ -172,6 +172,10 @@ class CpuTextIngestor : public TextIngestor {
     }
     return w;
   }
+  DeviceIngestSession* resident_session(const Cli&, std::string* error) override {
+    *error = "GPR_INGEST=cpu keeps no resident window";
+    return nullptr;
+  }
 };
 
 class UnsupportedSource : public WindowSource {
@@ -390,6 +394,11 @@ int Controller::run(WindowSource& src) {
   int ticks = 0;
   std::ofstream patch_out;
   if (args_.patch_out) patch_out.open(*args_.patch_out, std::ios::app);
+  if (snapshots_ && args_.daemon_mode) {
+    std::string line;
+    const bool ok = snapshots_->restore(&line);
+    log_.log(ok ? "INFO" : "WARN", line);
+  }
   auto next_tick = std::chrono::steady_clock::now();
   while (true) {
     if (args_.daemon_mode) {          // first tick fires immediately (tokio interval), main.rs:292-294
@@ -399,9 +408,11 @@ int Controller::run(WindowSource& src) {
     TickResult tr;
     const auto tick_t0 = std::chrono::steady_clock::now();
     double fetch_ms = 0;
+    bool resident = false;
     try {
       Window w = src.fetch(args_);
       fetch_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tick_t0).count();
+      resident = w.resident;
       tr = run_query_and_scale(w);
     } catch (const std::exception& e) {
       tr.ok = false;
@@ -425,6 +436,18 @@ int Controller::run(WindowSource& src) {
         j.set("body", rq.body);
         if (patch_out.is_open()) patch_out << j.dump() << "\n" << std::flush;
         else fprintf(stdout, "%s\n", j.dump().c_str());
+      }
+      // the verdict is out: now the window it was decided on may go to disk.  A failed write costs the next start
+      // the full range, nothing else — not the tick's result, not query_failures.
+      if (snapshots_ && resident) {
+        std::string line;
+        const int rc = snapshots_->save(&line);
+        if (rc > 0) {
+          log_.info(line);
+        } else if (rc < 0) {
+          ++snapshot_failures;
+          log_.counter("ERROR", "monotonic_counter.snapshot_failures", 1, "Snapshot not written: " + line);
+        }
       }
     } else {
       const size_t failures = consecutive_failures++;   // fetch_add returns the previous value

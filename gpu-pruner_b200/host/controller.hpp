@@ -18,6 +18,8 @@
 
 namespace gph {
 
+class DeviceIngestSession;
+
 // lib.rs:136-145
 struct PodMetricData {
   std::string name, ns, container, node_type, gpu_model;
@@ -90,6 +92,22 @@ class TextIngestor {
   // daemon mode: newest second of the window this ingestor keeps resident between ticks (0 = none: the next
   // tick must bring the full range).  An ingest with opt.slice_seconds > 0 may throw NeedFullWindow.
   virtual int64_t resident_t_end() const { return 0; }
+  // daemon mode: the session that keeps the window resident, for snapshots (snapshot.hpp); created if need be.
+  // nullptr (*error says why): this ingestor keeps no resident window, so there is nothing to snapshot.
+  virtual DeviceIngestSession* resident_session(const Cli&, std::string* error) {
+    *error = "this ingestor keeps no resident window";
+    return nullptr;
+  }
+};
+// --snapshot-file: the resident window saved after every tick and restored at start (snapshot.hpp make_file_snapshots).
+class WindowSnapshots {
+ public:
+  virtual ~WindowSnapshots() = default;
+  // before the first fetch: true = the window is resident again; *line says what was restored or why not
+  virtual bool restore(std::string* line) = 0;
+  // after a successful tick whose window is resident: 1 = written (*line describes it), 0 = nothing resident,
+  // -1 = the write failed (*line says why; the previous file is intact)
+  virtual int save(std::string* line) = 0;
 };
 class VerdictEngine {
  public:
@@ -120,8 +138,11 @@ class Controller {
   TickResult run_query_and_scale(const Window& w);
   // main.rs:286-330: one-shot or daemon loop with the consecutive-failure budget; returns exit code
   int run(WindowSource& src);
+  // --snapshot-file: restore before the first fetch, save after every successful tick with a resident window
+  void use_snapshots(WindowSnapshots* snapshots) { snapshots_ = snapshots; }
 
   uint64_t query_successes = 0, query_failures = 0, scale_successes = 0, scale_failures = 0;
+  uint64_t snapshot_failures = 0;
 
  private:
   Cli args_;
@@ -130,6 +151,7 @@ class Controller {
   Logger log_;
   Clock clock_;
   uint8_t enabled_;
+  WindowSnapshots* snapshots_ = nullptr;
 };
 
 }  // namespace gph

@@ -24,6 +24,7 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
  public:
   ~GprVerdictEngine() override {
     if (ctx_) {
+      free_exports();
       if (d_elig_) gpr_device_free(ctx_, d_elig_);
       if (d_created_) gpr_device_free(ctx_, d_created_);
       if (d_table_) gpr_device_free(ctx_, d_table_);
@@ -131,6 +132,11 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
 
   // ---- TextIngestor ---------------------------------------------------------------------------------
   int64_t resident_t_end() const override { return session_ ? session_->resident_t_end() : 0; }
+  DeviceIngestSession* resident_session(const Cli& args, std::string* error) override {
+    if (!ensure_ctx(args.gpu_device, error)) return nullptr;
+    if (!session_) session_.reset(new DeviceIngestSession(*this));
+    return session_.get();
+  }
 
   Window ingest(const Cli& args, const std::string& util, const std::string* prof, const std::string* power,
                 const IngestOptions& opt, std::string* note) override {
@@ -191,13 +197,7 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
     return more != 0;
   }
   void parse(int slot, std::vector<gpr_text_span>& spans, const TextGrid& grid, int plane) override {
-    gpr_text_grid g;
-    memset(&g, 0, sizeof g);
-    g.struct_size = sizeof g;
-    g.flags = (grid.fill ? GPR_TEXT_FILL : 0u) | (grid.resident ? GPR_TEXT_RESIDENT : 0u);
-    g.t_end = grid.t_end, g.window_seconds = grid.span, g.step = grid.step;
-    g.n_samples = grid.T, g.n_rows = grid.n_rows;
-    g.power_threshold = grid.power_threshold;
+    const gpr_text_grid g = text_grid(grid);
     check(gpr_text_parse(ctx_, slot, spans.data(), (uint32_t)spans.size(), &g, plane), "gpr_text_parse");
   }
   void patch_row(int plane, uint32_t row, uint32_t T, const float* data, uint32_t n_newest, bool resident) override {
@@ -223,6 +223,100 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
     check(gpr_resident_init(ctx_, pods, G, T, with_power ? GPR_F_POWER_PLANE : 0u), "gpr_resident_init");
   }
   void resident_advance(uint32_t n_new) override { check(gpr_resident_advance(ctx_, n_new), "gpr_resident_advance"); }
+  // Snapshots: the encoder writes into device buffers kept across ticks, then one copy per array lands in pinned host
+  // memory (the two are timed apart).  Capacities carry a quarter of head-room, so a steady tick encodes once; a
+  // grown ring is sized by the first call (GPR_E_CAPACITY returns the true counts) and encoded again.
+  struct ExportBufs {
+    void* d = nullptr;  // series_chunks | chunk_bytes | rows | data, on the device
+    void* h = nullptr;  // the same, pinned host memory
+    uint64_t cap_series = 0, cap_chunks = 0, cap_bytes = 0;
+    size_t bytes() const { return (cap_series + 1) * 8 + (cap_chunks + 1) * 8 + cap_series * 4 + cap_bytes; }
+  };
+  void free_exports() {
+    for (ExportBufs& b : xb_) {
+      if (b.d) gpr_device_free(ctx_, b.d);
+      if (b.h) gpr_host_free(ctx_, b.h);
+      b = ExportBufs();
+    }
+  }
+  void grow_export(ExportBufs& b, uint64_t series, uint64_t chunks, uint64_t bytes) {
+    if (b.d) gpr_device_free(ctx_, b.d), b.d = nullptr;
+    if (b.h) gpr_host_free(ctx_, b.h), b.h = nullptr;
+    b.cap_series = series + series / 4 + 64, b.cap_chunks = chunks + chunks / 4 + 64, b.cap_bytes = bytes + bytes / 4 + 4096;
+    check(gpr_device_alloc(ctx_, b.bytes(), &b.d), "snapshot buffer");
+    check(gpr_host_alloc(ctx_, b.bytes(), &b.h), "snapshot buffer");
+  }
+  static gpr_text_grid text_grid(const TextGrid& grid) {
+    gpr_text_grid g;
+    memset(&g, 0, sizeof g);
+    g.struct_size = sizeof g;
+    g.flags = (grid.fill ? GPR_TEXT_FILL : 0u) | (grid.resident ? GPR_TEXT_RESIDENT : 0u);
+    g.t_end = grid.t_end, g.window_seconds = grid.span, g.step = grid.step;
+    g.n_samples = grid.T, g.n_rows = grid.n_rows;
+    g.power_threshold = grid.power_threshold;
+    return g;
+  }
+  void resident_export(int plane, const TextGrid& grid, ChunkPlaneView* out, double* export_ms, double* copy_ms) override {
+    ExportBufs& b = xb_[plane];
+    const gpr_text_grid g = text_grid(grid);
+    const auto t0 = std::chrono::steady_clock::now();
+    if (!b.d) grow_export(b, 0, 0, 0);
+    gpr_chunk_export x;
+    for (int attempt = 0;; ++attempt) {
+      unsigned char* d = static_cast<unsigned char*>(b.d);
+      memset(&x, 0, sizeof x);
+      x.struct_size = sizeof x;
+      x.mem_kind = GPR_MEM_DEVICE;
+      x.series_chunks = reinterpret_cast<uint64_t*>(d);
+      x.chunk_bytes = reinterpret_cast<uint64_t*>(d + (b.cap_series + 1) * 8);
+      x.rows = reinterpret_cast<uint32_t*>(d + (b.cap_series + 1) * 8 + (b.cap_chunks + 1) * 8);
+      x.data = d + (b.cap_series + 1) * 8 + (b.cap_chunks + 1) * 8 + b.cap_series * 4;
+      x.cap_series = b.cap_series, x.cap_chunks = b.cap_chunks, x.cap_bytes = b.cap_bytes;
+      const int rc = gpr_resident_export(ctx_, &g, plane, 120, &x);
+      if (rc == GPR_E_CAPACITY && attempt == 0) {
+        grow_export(b, x.n_series, x.n_chunks, x.n_bytes);
+        continue;
+      }
+      check(rc, "gpr_resident_export");
+      break;
+    }
+    const auto t1 = std::chrono::steady_clock::now();
+    unsigned char* d = static_cast<unsigned char*>(b.d);
+    unsigned char* h = static_cast<unsigned char*>(b.h);
+    const size_t o_cb = (b.cap_series + 1) * 8, o_rows = o_cb + (b.cap_chunks + 1) * 8, o_data = o_rows + b.cap_series * 4;
+    check(gpr_memcpy(ctx_, h, d, (x.n_series + 1) * 8, GPR_MEM_HOST, GPR_MEM_DEVICE), "snapshot copy");
+    check(gpr_memcpy(ctx_, h + o_cb, d + o_cb, (x.n_chunks + 1) * 8, GPR_MEM_HOST, GPR_MEM_DEVICE), "snapshot copy");
+    if (x.n_series) check(gpr_memcpy(ctx_, h + o_rows, d + o_rows, x.n_series * 4, GPR_MEM_HOST, GPR_MEM_DEVICE), "snapshot copy");
+    if (x.n_bytes) check(gpr_memcpy(ctx_, h + o_data, d + o_data, x.n_bytes, GPR_MEM_HOST, GPR_MEM_DEVICE), "snapshot copy");
+    const auto t2 = std::chrono::steady_clock::now();
+    out->n_series = x.n_series, out->n_chunks = x.n_chunks, out->n_bytes = x.n_bytes;
+    out->series_chunks = reinterpret_cast<const uint64_t*>(h);
+    out->chunk_bytes = reinterpret_cast<const uint64_t*>(h + o_cb);
+    out->rows = reinterpret_cast<const uint32_t*>(h + o_rows);
+    out->data = h + o_data;
+    *export_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
+    *copy_ms = std::chrono::duration<double, std::milli>(t2 - t1).count();
+  }
+  // The planes go up as host batches: gpr_chunks_scatter checks and merges them in pieces through its own staging,
+  // so the file's buffer needs no device copy of itself.  The binary's ring has no block index (no GPR_F_BLOCK_INDEX),
+  // so there is nothing to reindex.
+  void resident_restore(uint32_t pods, uint32_t G, uint32_t T, bool with_power, const ChunkPlaneView planes[2],
+                        const TextGrid& grid) override {
+    resident_init(pods, G, T, with_power);
+    for (int k = 0; k < (with_power ? 2 : 1); ++k) {
+      const ChunkPlaneView& v = planes[k];
+      gpr_chunk_batch cb;
+      memset(&cb, 0, sizeof cb);
+      cb.struct_size = sizeof cb;
+      cb.mem_kind = GPR_MEM_HOST;
+      cb.series_chunks = v.series_chunks, cb.rows = v.rows, cb.chunk_bytes = v.chunk_bytes, cb.data = v.data;
+      cb.n_series = (uint32_t)v.n_series;
+      TextGrid pg = grid;
+      pg.power_threshold = k == 1 ? grid.power_threshold : 0.0;
+      const gpr_text_grid g = text_grid(pg);
+      check(gpr_chunks_scatter(ctx_, &cb, &g, k, nullptr), k == 0 ? "gpr_chunks_scatter (util plane)" : "gpr_chunks_scatter (power plane)");
+    }
+  }
   const float* plane(int plane) override {
     float *u = nullptr, *p = nullptr;
     check(gpr_text_planes(ctx_, &u, &p), "gpr_text_planes");
@@ -299,6 +393,7 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
   void drop() {
     if (!ctx_) return;
     session_.reset();  // its resident window dies with the context
+    free_exports();
     if (d_elig_) gpr_device_free(ctx_, d_elig_), d_elig_ = nullptr;
     if (d_created_) gpr_device_free(ctx_, d_created_), d_created_ = nullptr;
     if (d_table_) gpr_device_free(ctx_, d_table_), d_table_ = nullptr;
@@ -326,6 +421,7 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
 
   gpr_ctx* ctx_ = nullptr;
   std::unique_ptr<DeviceIngestSession> session_;
+  ExportBufs xb_[2];
   uint64_t cap_cells_ = 0;
   bool cap_power_ = false;
   void* d_elig_ = nullptr;

@@ -559,6 +559,68 @@ Window DeviceIngestSession::ingest(const std::string& util, const std::string* p
   return out;
 }
 
+bool DeviceIngestSession::save_state(SnapshotState* out) const {
+  const State& st = *st_;
+  if (!st.valid || !st.asg) return false;
+  const Window& w = st.w;
+  SnapshotState& s = *out;
+  s = SnapshotState();
+  s.span = w.span, s.step = w.step, s.t_end = w.t_end;
+  s.T = w.T, s.pods_cap = st.pods_cap, s.G = w.G;
+  s.with_power = st.with_power, s.power_threshold = st.power_threshold;
+  s.pods.assign(w.pods.begin(), w.pods.end());
+  st.asg->each_known([&](uint64_t h1, uint64_t h2, Assigner::Result r, uint32_t pod, uint32_t slot) {
+    s.known.push_back(SnapshotState::Known{h1, h2, (uint32_t)r, pod, slot});
+  });
+  s.power_keys = st.asg->power_keys();
+  s.power_keys.resize(s.pods.size());
+  s.prof_sigs.assign(st.asg->prof_sigs().begin(), st.asg->prof_sigs().end());
+  s.prof_rows = st.prof_rows;
+  return true;
+}
+
+void DeviceIngestSession::export_planes(ChunkPlaneView planes[2], double* export_ms, double* copy_ms) {
+  const State& st = *st_;
+  if (!st.valid) throw std::logic_error("nothing resident to export");
+  TextDevice::TextGrid grid;
+  grid.t_end = st.w.t_end, grid.span = st.w.span, grid.step = st.w.step, grid.T = st.w.T;
+  grid.n_rows = st.pods_cap * st.w.G, grid.fill = false, grid.resident = true;
+  *export_ms = *copy_ms = 0;
+  planes[0] = planes[1] = ChunkPlaneView();
+  for (int k = 0; k < (st.with_power ? 2 : 1); ++k) {
+    grid.power_threshold = k == 1 ? st.power_threshold : 0.0;
+    double e = 0, c = 0;
+    dev_.resident_export(k, grid, &planes[k], &e, &c);
+    *export_ms += e, *copy_ms += c;
+  }
+}
+
+void DeviceIngestSession::restore_state(const SnapshotState& s, const ChunkPlaneView planes[2]) {
+  State& st = *st_;
+  st.valid = false;
+  st.w = Window();
+  st.asg.reset(new Assigner(st.w));
+  st.prof_rows.clear();
+  TextDevice::TextGrid grid;
+  grid.t_end = s.t_end, grid.span = s.span, grid.step = s.step, grid.T = s.T;
+  grid.n_rows = s.pods_cap * s.G, grid.fill = false, grid.resident = true;
+  grid.power_threshold = s.power_threshold;
+  dev_.resident_restore(s.pods_cap, s.G, s.T, s.with_power, planes, grid);  // throws: the session stays cold
+  Window& w = st.w;
+  for (const PodEntry& pe : s.pods) w.pods.push_back(pe);
+  w.P = (uint32_t)s.pods.size(), w.G = s.G, w.T = s.T;
+  w.t_end = s.t_end, w.step = s.step, w.span = s.span;
+  std::map<std::pair<uint32_t, uint32_t>, std::vector<std::string>> sigs(s.prof_sigs.begin(), s.prof_sigs.end());
+  st.asg->adopt_pods(s.power_keys, std::move(sigs));
+  for (const SnapshotState::Known& k : s.known)
+    st.asg->insert_known(k.h1, k.h2, (Assigner::Result)k.result, k.pod, k.slot);
+  st.pods_cap = s.pods_cap;
+  st.with_power = s.with_power;
+  st.power_threshold = s.power_threshold;
+  st.prof_rows = s.prof_rows;
+  st.valid = true;
+}
+
 Window ingest_matrix_device(TextDevice& dev, const std::string& util, const std::string* prof,
                             const std::string* power, const IngestOptions& opt, DeviceIngestReport* report) {
   DeviceIngestSession once(dev);

@@ -12,6 +12,7 @@
 
 #include "../../include/gpr.h"
 #include "ingest.hpp"
+#include "snapshot.hpp"
 
 namespace gph {
 
@@ -50,6 +51,22 @@ class TextDevice {
   // daemon mode: (re)create the resident ring [rows][T] (all "no sample"), and open the next n_new buckets
   virtual void resident_init(uint32_t pods, uint32_t G, uint32_t T, bool with_power) = 0;
   virtual void resident_advance(uint32_t n_new) = 0;
+  // daemon-mode snapshots (snapshot.hpp): plane `plane` of the resident ring as Prometheus XOR chunks of at most 120
+  // samples (gpr_resident_export), in host memory the device keeps until its next export of that plane; the time spent
+  // encoding and copying out goes to *export_ms / *copy_ms.  A device that cannot snapshot throws (save_snapshot then
+  // reports a failed write; restore_snapshot a refused snapshot).
+  virtual void resident_export(int plane, const TextGrid& grid, ChunkPlaneView* out, double* export_ms,
+                               double* copy_ms) {
+    (void)plane, (void)grid, (void)out, (void)export_ms, (void)copy_ms;
+    throw std::logic_error("this device keeps no snapshots");
+  }
+  // a fresh ring of the given shape (resident_init) holding the exported planes (planes[1] only with_power), merged in
+  // by gpr_chunks_scatter(GPR_TEXT_RESIDENT) on `grid`; throws if a plane is refused
+  virtual void resident_restore(uint32_t pods, uint32_t G, uint32_t T, bool with_power, const ChunkPlaneView planes[2],
+                                const TextGrid& grid) {
+    (void)pods, (void)G, (void)T, (void)with_power, (void)planes, (void)grid;
+    throw std::logic_error("this device keeps no snapshots");
+  }
 };
 
 struct DeviceIngestReport {
@@ -82,6 +99,14 @@ class DeviceIngestSession {
   // newest second the resident window holds (0 = nothing resident): the next delta must start right after it
   int64_t resident_t_end() const;
   void invalidate();
+  // Snapshots of the session between ticks (snapshot.hpp).  save_state: false = nothing resident.  export_planes: the
+  // ring's planes through the device (planes[1] only with a power plane).  restore_state: the ring first, through the
+  // device, then the session; the session is valid only once both are in place — if the device refuses a plane (it
+  // throws) the session stays cold and the next tick takes the full range.  The existing delta checks then decide
+  // whether the first slice can be absorbed.
+  bool save_state(SnapshotState* out) const;
+  void export_planes(ChunkPlaneView planes[2], double* export_ms, double* copy_ms);
+  void restore_state(const SnapshotState& s, const ChunkPlaneView planes[2]);
 
  private:
   struct State;

@@ -194,6 +194,37 @@ class Assigner {
   }
   void count_skipped() { ++w_.stats.series_skipped; }
 
+  // Daemon-mode snapshots (snapshot.hpp): what lives beyond one tick, and its restore into a fresh Assigner whose
+  // window already holds the pods.  The pod table is rebuilt from the pods, not stored.  The identities stay valid
+  // across processes because hash128 depends on the label bytes alone (a change to it changes kSnapshotVersion).
+  template <typename F>
+  void each_known(F&& f) const {
+    for (const Known& k : known_)
+      if (k.h1 || k.h2) f(k.h1, k.h2, k.result, k.pod, k.slot);
+  }
+  const std::vector<std::vector<uint64_t>>& power_keys() const { return power_keys_; }
+  const std::map<std::pair<uint32_t, uint32_t>, std::vector<std::string>>& prof_sigs() const { return prof_sigs_; }
+  void adopt_pods(std::vector<std::vector<uint64_t>> power_keys,
+                  std::map<std::pair<uint32_t, uint32_t>, std::vector<std::string>> prof_sigs) {
+    const size_t P = w_.pods.size();
+    size_t cap = 1024;
+    while (P * 2 > cap) cap *= 4;  // the load factor find_or_add_pod keeps
+    table_.assign(cap, 0);
+    pod_hash_.clear();
+    const size_t mask = cap - 1;
+    for (size_t q = 0; q < P; ++q) {
+      const PodEntry& pe = static_cast<const PodList&>(w_.pods)[q];
+      const uint64_t h = hash_bytes(hash_bytes(0xcbf29ce484222325ull, pe.name), pe.ns);  // as extract_fields
+      pod_hash_.push_back(h);
+      size_t j = (size_t)(h ^ (h >> 32)) & mask;
+      while (table_[j]) j = (j + 1) & mask;
+      table_[j] = (uint32_t)q + 1;
+    }
+    power_keys_ = std::move(power_keys);
+    power_keys_.resize(P);
+    prof_sigs_ = std::move(prof_sigs);
+  }
+
   // Daemon mode: the same series comes back every tick and must keep its row.  A series is identified by the
   // bytes of its label map as the server prints them (sorted keys, so the text is canonical) plus the plane it
   // feeds; known series skip the label work altogether.

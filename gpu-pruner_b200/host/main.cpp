@@ -10,6 +10,7 @@
 #include "controller.hpp"
 #include "kube.hpp"
 #include "promql.hpp"
+#include "snapshot.hpp"
 
 int main(int argc, char** argv) {
   std::vector<std::string> args(argv + 1, argv + argc);
@@ -41,5 +42,24 @@ int main(int argc, char** argv) {
   if (ing && std::string(ing) == "cpu") cpu_ingestor = gph::make_cpu_text_ingestor(), ingestor = cpu_ingestor.get();
   std::unique_ptr<gph::WindowSource> src = gph::make_window_source(cli.prometheus_url, ingestor, &log);
   gph::Controller ctl(cli, kube.get(), engine.get(), log, gph::system_clock());
+  // --snapshot-file: the resident window survives a restart (snapshot.hpp).  The CPU ingest keeps no resident window,
+  // so there is nothing to save: said once, and the run is the one without the flag.
+  std::unique_ptr<gph::WindowSnapshots> snapshots;
+  if (cli.snapshot_file) {
+    std::string why;
+    if (!ingestor->resident_session(cli, &why)) {
+      log.warn("--snapshot-file ignored: snapshots need the device ingest (" + why + ")");
+    } else {
+      gph::SnapshotKey key;
+      key.span = cli.duration * 60;
+      const bool want_power = cli.power_threshold && *cli.power_threshold != 0.0;
+      key.power_threshold = want_power ? *cli.power_threshold : 0.0;   // as FileSource ingests the power plane
+      key.selectors[0] = sel.util, key.selectors[1] = sel.prof, key.selectors[2] = sel.power;
+      snapshots = gph::make_file_snapshots(*cli.snapshot_file, key, [ingestor, &cli](std::string* error) {
+        return ingestor->resident_session(cli, error);
+      });
+      ctl.use_snapshots(snapshots.get());
+    }
+  }
   return ctl.run(*src);
 }
