@@ -240,6 +240,7 @@ struct gpr_ctx {
   Buf<float> d_res_next[4];
   Buf<uint32_t> d_remap_map;            // a host map, uploaded
   Buf<unsigned int> d_remap_check;      // a device map's check: [first bad new row | seen bitmap | dup bitmap]
+  Buf<uint32_t> d_live;                 // gpr_resident_live_rows' bitmap for a host destination
 
   // device-side ingest of response text (gpr_text_scan / gpr_text_parse)
   Buf<uint8_t> d_text[3];
@@ -1485,6 +1486,36 @@ int gpr_resident_remap(gpr_ctx* ctx, uint32_t n_pods, uint32_t n_gpus, const uin
   for (int k = 0; k < 4; ++k) cur[k]->swap(ctx->d_res_next[k]);
   ctx->res_P = n_pods, ctx->res_G = n_gpus;
   for (Buf<float>& b : ctx->d_res_next) CU(b.release());  // the old ring
+  return GPR_OK;
+  GPR_CATCH(ctx)
+}
+
+int gpr_resident_live_rows(gpr_ctx* ctx, uint32_t* bits, int32_t mem_kind) {
+  if (!ctx) return GPR_E_INVALID;
+  GPR_TRY
+  NvtxRange nvtx_range("gpr_resident_live_rows");
+  if (const int rc = enter(ctx)) return rc;
+  if (!ctx->d_res_util) return fail(ctx, GPR_E_STATE, "no resident window (gpr_resident_init)");
+  if (!bits) return fail(ctx, GPR_E_INVALID, "bits is NULL");
+  if (mem_kind != GPR_MEM_HOST && mem_kind != GPR_MEM_DEVICE) return fail(ctx, GPR_E_INVALID, "bad mem_kind %d", mem_kind);
+  const uint32_t rows = ctx->res_P * ctx->res_G, words = (rows + 31) / 32;
+  // a current index answers from 1/64 of the bytes (its block maxima are NaN exactly where a block has no sample); a
+  // stale one is not read, and not refused either: this call only reads
+  const bool index = gpr::live_rows_from_index(ctx->d_idx_util != nullptr, ctx->idx_stale);
+  const float* p0 = index ? ctx->d_idx_util : ctx->d_res_util;
+  const float* p1 = index ? ctx->d_idx_power : ctx->d_res_power;
+  const uint32_t len = index ? ctx->idx_ld : ctx->res_T;
+  uint32_t* out = bits;
+  if (mem_kind == GPR_MEM_HOST) {
+    CU(ctx->d_live.grow(ctx->stream, words));
+    out = ctx->d_live;
+  }
+  const int rc = launch(ctx, gpr::k_live_rows, gpr::live_rows_grid(rows, ctx->sm_count), gpr::kRingThreads, 0, false,
+                        reinterpret_cast<const uint32_t*>(p0), reinterpret_cast<const uint32_t*>(p1), rows, len, out);
+  if (rc != GPR_OK) return rc;
+  if (mem_kind == GPR_MEM_HOST)
+    CU(cudaMemcpyAsync(bits, out, (size_t)words * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
   return GPR_OK;
   GPR_CATCH(ctx)
 }

@@ -5,7 +5,7 @@
 // gpr_resident_advance (which source columns survive, where they land, what each plane gets, the grid, the index
 // row length) is plain functions.  gpr_api.cu launches what these return; tests/cpp/ring_emul.cpp runs the same
 // source on the CPU against a numpy model of the ring.  gpr_resident_remap's row gather and map check are here too
-// (tests/cpp/remap_emul.cpp).
+// (tests/cpp/remap_emul.cpp), and gpr_resident_live_rows' row test (tests/cpp/live_rows_emul.cpp).
 #pragma once
 
 #include <stddef.h>
@@ -210,6 +210,80 @@ __global__ void __launch_bounds__(kRingThreads) k_remap_rows(uint32_t* __restric
     } else {
       for (uint32_t j = threadIdx.x; j < len; j += blockDim.x) out[j] = in ? in[j] : kNoSampleBits;
     }
+  }
+}
+
+// ---- gpr_resident_live_rows: which rows hold at least one sample
+constexpr uint32_t kLiveWarps = kRingThreads / 32;  // warps of a k_live_rows CTA, 32 rows (one bitmap word) each
+
+// CTAs of k_live_rows: one bitmap word per warp and round, as many CTAs as ring_grid gives for that many CTA rounds
+inline uint32_t live_rows_grid(size_t rows, int sm_count) {
+  const size_t words = (rows + 31) / 32;
+  return ring_grid(std::max<size_t>(1, (words + kLiveWarps - 1) / kLiveWarps), sm_count);
+}
+
+// what gpr_resident_live_rows reads: a current block index (1/64 of the bytes) if the ring has one, else the planes
+inline bool live_rows_from_index(bool has_index, bool index_stale) { return has_index && !index_stale; }
+
+// every NaN is "no sample" (gpr_resident_planes writers and gpr_append columns may store other NaNs than the fill)
+__device__ __forceinline__ bool has_sample_bits(uint32_t b) { return (b & 0x7FFFFFFFu) <= 0x7F800000u; }
+
+// One warp: does the row of `len` cells hold a cell that is not NaN?  The answer is the same on every lane.  The reads
+// stop at the first step that finds one: the first step is one coalesced load per lane (a live row usually ends
+// there), later steps issue four independent loads per lane so that a row without a sample is read at full rate.
+// 16-byte loads when rows start on a 16-byte boundary (len % 4 == 0), 4-byte ones otherwise.
+__device__ __forceinline__ bool row_has_sample(const uint32_t* __restrict__ row, uint32_t len, int lane) {
+  if (len % 4u == 0) {
+    const uint4* r4 = reinterpret_cast<const uint4*>(row);
+    const uint32_t n4 = len / 4u;
+    uint32_t per = 1;
+    for (uint32_t base = 0; base < n4; base += 32u * per, per = 4) {
+      bool hit = false;
+#pragma unroll
+      for (uint32_t u = 0; u < 4; ++u) {
+        const uint32_t k = base + u * 32u + (uint32_t)lane;
+        if (u < per && k < n4) {
+          const uint4 v = r4[k];
+          hit |= has_sample_bits(v.x) || has_sample_bits(v.y) || has_sample_bits(v.z) || has_sample_bits(v.w);
+        }
+      }
+      if (__ballot_sync(0xFFFFFFFFu, hit)) return true;
+    }
+    return false;
+  }
+  uint32_t per = 1;
+  for (uint32_t base = 0; base < len; base += 32u * per, per = 4) {
+    bool hit = false;
+#pragma unroll
+    for (uint32_t u = 0; u < 4; ++u) {
+      const uint32_t k = base + u * 32u + (uint32_t)lane;
+      if (u < per && k < len) hit |= has_sample_bits(row[k]);
+    }
+    if (__ballot_sync(0xFFFFFFFFu, hit)) return true;
+  }
+  return false;
+}
+
+// Bit r of bits[r / 32] = row r holds a cell that is not NaN in p0 or, if given, p1 (rows of `len` cells: the planes
+// with len = T, or their block index with len = idx_ld, whose padding is NaN).  A warp owns a word: it reads its 32
+// rows one after the other, lane i keeps row i's answer, and one ballot makes the word.  Padding bits are zero, every
+// word is written once, no atomics.  Grid: live_rows_grid.
+__global__ void __launch_bounds__(kRingThreads) k_live_rows(const uint32_t* __restrict__ p0,
+                                                            const uint32_t* __restrict__ p1, uint32_t n_rows,
+                                                            uint32_t len, uint32_t* __restrict__ bits) {
+  const int lane = threadIdx.x & 31;
+  const uint32_t n_words = (n_rows + 31u) / 32u, n_warps = gridDim.x * (blockDim.x >> 5);
+  for (uint32_t w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); w < n_words; w += n_warps) {
+    const uint32_t r0 = w * 32u, n = min(32u, n_rows - r0);
+    bool mine = false;
+    for (uint32_t i = 0; i < n; ++i) {
+      const size_t r = (size_t)r0 + i;
+      bool live = row_has_sample(p0 + r * len, len, lane);
+      if (!live && p1) live = row_has_sample(p1 + r * len, len, lane);
+      if ((uint32_t)lane == i) mine = live;
+    }
+    const uint32_t word = __ballot_sync(0xFFFFFFFFu, mine);
+    if (lane == 0) bits[w] = word;
   }
 }
 

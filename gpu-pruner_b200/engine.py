@@ -280,6 +280,7 @@ class IdleEngine:
     def resident_init(self, P: int, G: int, T: int, power_plane: bool = False, block_index: bool = False):
         flags = (ffi.GPR_F_POWER_PLANE if power_plane else 0) | (ffi.GPR_F_BLOCK_INDEX if block_index else 0)
         self._check(self._lib.gpr_resident_init(self._h, P, G, T, flags))
+        self._res_rows = int(P) * int(G)
 
     def resident_reindex(self):
         self._check(self._lib.gpr_resident_reindex(self._h))
@@ -557,11 +558,24 @@ class IdleEngine:
                 raise ValueError(f"src_rows must be a contiguous tensor of P * G = {P * G} entries")
             self._check(self._lib.gpr_resident_remap(self._h, int(P), int(G), src_rows.data_ptr(),
                                                      ffi.GPR_MEM_DEVICE))
+            self._res_rows = int(P) * int(G)
             return
         rows = np.ascontiguousarray(src_rows, dtype=np.uint32).ravel()
         if rows.size != P * G:
             raise ValueError(f"src_rows has {rows.size} entries, not P * G = {P * G}")
         self._check(self._lib.gpr_resident_remap(self._h, int(P), int(G), rows.ctypes.data, ffi.GPR_MEM_HOST))
+        self._res_rows = int(P) * int(G)
+
+    def resident_live_rows(self) -> np.ndarray:
+        """Which rows of the resident ring hold at least one sample (any non-NaN cell) in the util plane or the power
+        plane (gpr_resident_live_rows): a bool array of ``P * G`` entries, row ``pod * G + slot``.  What a caller of
+        :meth:`resident_remap` reads to choose which pods to keep."""
+        rows = getattr(self, "_res_rows", None)
+        if rows is None:
+            raise RuntimeError("no resident window (resident_init)")
+        words = np.zeros(max(1, (rows + 31) // 32), np.uint32)
+        self._check(self._lib.gpr_resident_live_rows(self._h, words.ctypes.data, ffi.GPR_MEM_HOST))
+        return np.unpackbits(words.view(np.uint8), bitorder="little")[:rows].astype(bool)
 
     def text_planes(self):
         u, w = C.c_void_p(), C.c_void_p()

@@ -43,6 +43,7 @@ std::string usage() {
       "      --print-query                          (extension) print the rendered PromQL and exit\n"
       "      --gpu-device <N>                       (extension) CUDA device ordinal [default: 0]\n"
       "      --snapshot-file <PATH>                 (extension) with -d: save the resident window after every tick, resume from it at start\n"
+      "      --reshape-ring                         (extension) with -d: reshape the resident window on the GPU when pods or GPU slots outgrow it\n"
       "  -h, --help                                 Print help\n";
 }
 
@@ -138,6 +139,7 @@ ParseOutcome parse_cli(const std::vector<std::string>& args) {
     return e;
   }};
   specs["snapshot-file"] = {0, true, [&](const std::string& v) { c.snapshot_file = v; return std::string(); }};
+  specs["reshape-ring"] = {0, false, [&](const std::string&) { c.reshape_ring = true; return std::string(); }};
   specs["now"] = {0, true, [&](const std::string& v) { return parse_i64(v, &c.now_override); }};
   specs["max-ticks"] = {0, true, [&](const std::string& v) {
     int64_t x;
@@ -202,6 +204,8 @@ ParseOutcome parse_cli(const std::vector<std::string>& args) {
   }
   if (c.snapshot_file && !c.daemon_mode)
     return fail("the argument '--snapshot-file <PATH>' can only be used with '--daemon-mode'");
+  if (c.reshape_ring && !c.daemon_mode)
+    return fail("the argument '--reshape-ring' can only be used with '--daemon-mode'");
   if (!have_url && !c.print_query)
     return fail("the following required arguments were not provided:\n  --prometheus-url <PROMETHEUS_URL>");
   out.ok = true;

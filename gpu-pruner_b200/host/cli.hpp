@@ -39,6 +39,9 @@ struct Cli {
   int max_ticks = 0;                          // --max-ticks N (tests): stop the daemon loop after N ticks
   std::optional<std::string> snapshot_file;   // --snapshot-file PATH (-d only): save the resident window after every
                                               // tick, resume from it at start (DESIGN.md §8i)
+  bool reshape_ring = false;                  // --reshape-ring (-d only): a tick whose cluster outgrew the resident
+                                              // window's shape reshapes it on the GPU instead of querying the full
+                                              // range (DESIGN.md §8e)
 };
 
 struct ParseOutcome {

@@ -133,6 +133,7 @@ class FileSource : public WindowSource {
     }
     opt.slice_seconds = slice_seconds;
     opt.resident = resident;
+    opt.reshape = args.reshape_ring;
     if (log_) {
       char rbuf[160];
       snprintf(rbuf, sizeof rbuf, "Recorded responses read from %s: %.1f MB in %.1f ms", d.c_str(), read_bytes / 1e6,
@@ -145,6 +146,8 @@ class FileSource : public WindowSource {
     } else {
       std::string note;
       w = ingestor_->ingest(args, util, pprof, ppower, opt, &note);
+      if (log_ && !w.stats.ring_reshape.empty())  // --reshape-ring: one line per reshape, with its counter
+        log_->counter("INFO", "monotonic_counter.ring_reshapes", 1, w.stats.ring_reshape);
       if (log_ && !note.empty()) log_->info(note);
     }
     // node_type for the rows of PodMetricData: the node_dmi_info join of query.promql.j2:23-34

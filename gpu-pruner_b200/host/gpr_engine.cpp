@@ -221,8 +221,18 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
   }
   void resident_init(uint32_t pods, uint32_t G, uint32_t T, bool with_power) override {
     check(gpr_resident_init(ctx_, pods, G, T, with_power ? GPR_F_POWER_PLANE : 0u), "gpr_resident_init");
+    resident_rows_ = pods * G;
   }
   void resident_advance(uint32_t n_new) override { check(gpr_resident_advance(ctx_, n_new), "gpr_resident_advance"); }
+  // --reshape-ring: the map goes up from the host (gpr_resident_remap checks it there), the bitmap comes back to it
+  void resident_remap(uint32_t pods, uint32_t G, const std::vector<uint32_t>& src_rows) override {
+    check(gpr_resident_remap(ctx_, pods, G, src_rows.data(), GPR_MEM_HOST), "gpr_resident_remap");
+    resident_rows_ = pods * G;
+  }
+  void resident_live_rows(std::vector<uint32_t>* bits) override {
+    bits->assign(((size_t)resident_rows_ + 31) / 32, 0u);
+    check(gpr_resident_live_rows(ctx_, bits->data(), GPR_MEM_HOST), "gpr_resident_live_rows");
+  }
   // Snapshots: the encoder writes into device buffers kept across ticks, then one copy per array lands in pinned host
   // memory (the two are timed apart).  Capacities carry a quarter of head-room, so a steady tick encodes once; a
   // grown ring is sized by the first call (GPR_E_CAPACITY returns the true counts) and encoded again.
@@ -422,6 +432,7 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
   gpr_ctx* ctx_ = nullptr;
   std::unique_ptr<DeviceIngestSession> session_;
   ExportBufs xb_[2];
+  uint32_t resident_rows_ = 0;  // rows of the resident ring (pods x G)
   uint64_t cap_cells_ = 0;
   bool cap_power_ = false;
   void* d_elig_ = nullptr;

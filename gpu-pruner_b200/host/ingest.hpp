@@ -69,6 +69,8 @@ struct IngestStats {
   uint64_t series_in = 0, series_skipped = 0, samples_in = 0, samples_out_of_window = 0,
            duplicates_merged = 0, tiny_values_clamped = 0;
   std::vector<std::string> warnings;
+  // daemon mode with IngestOptions::reshape: what reshaping the resident ring did this tick ("" = it was not reshaped)
+  std::string ring_reshape;
 };
 
 struct Window {
@@ -102,6 +104,10 @@ struct IngestOptions {
   // veto agrees with Prometheus' float64 `x >= threshold` (include/gpr.h, gpr_window.power_threshold).
   // 0 / NaN = no power clause: plain rounding
   double power_threshold = 0.0;
+  // daemon mode (--reshape-ring): a delta tick whose pods outgrow the ring's rows, or whose pod gains a series slot
+  // beyond its G, reshapes the ring on the GPU (gpr_resident_live_rows + gpr_resident_remap) instead of throwing
+  // NeedFullWindow; pods without a sample left in the window are dropped then
+  bool reshape = false;
 };
 
 // thrown by a delta ingest when the resident state cannot absorb the tick (new GPU slot beyond the ring's shape,

@@ -346,6 +346,60 @@ void plan_text(TextDevice& dev, TextPlan& plan, Assigner& asg, Window& w, bool i
   if (skip_trailing_ws(t, at) != t.size()) throw NotCompact{"trailing bytes after the response"};
 }
 
+// IngestOptions::reshape: a delta tick whose pods outgrew the ring's rows (`pods_cap`) or whose pod gained a slot
+// beyond w.G.  The tick's buckets are open already (resident_advance), so a pod whose last sample aged out with this
+// tick has no live row.  Kept: every pod with a live row in either plane, or with a series in this tick's slice; the
+// others are dropped.  The new shape applies the full rebuild's head-room rule to the kept pods, and G never shrinks:
+// [kept + kept / 4 + 64][max(G, slots needed)].  Kept pod `slot` moves to `slot'` with its rows
+// (src_rows[slot' * G' + g] = slot * G + g), a pod that joined this tick starts without a sample.  Then everything
+// that names a pod or a row is renumbered: the pods, the Assigner (pod table, known series, power keys, PROF
+// signatures), the session's PROF rows and this tick's series.  Returns the log line.
+std::string reshape_ring(TextDevice& dev, Window& w, Assigner& asg, uint32_t* pods_cap,
+                         std::vector<std::pair<uint32_t, uint32_t>>* prof_rows, TextPlan* plans, int n_plans) {
+  const uint32_t P_old = *pods_cap, G_old = w.G, n_pods = (uint32_t)w.pods.size();
+  const auto t0 = std::chrono::steady_clock::now();
+  std::vector<uint32_t> bits;
+  dev.resident_live_rows(&bits);
+  const double live_ms = ms_since(t0);
+  if (bits.size() < ((size_t)P_old * G_old + 31) / 32) throw std::logic_error("live-row bitmap shorter than the ring");
+  std::vector<uint8_t> keep(n_pods, 0);
+  for (uint32_t p = 0; p < std::min(n_pods, P_old); ++p)
+    for (uint32_t g = 0; g < G_old && !keep[p]; ++g) {
+      const size_t r = (size_t)p * G_old + g;
+      keep[p] = (uint8_t)((bits[r >> 5] >> (r & 31)) & 1u);
+    }
+  for (int k = 0; k < n_plans; ++k)
+    for (const DevSeries& s : plans[k].series) keep[s.pod] = 1;
+  std::vector<uint32_t> to(n_pods, Assigner::kDropped);
+  uint32_t kept = 0, G_new = G_old;
+  const PodList& pods = w.pods;
+  for (uint32_t p = 0; p < n_pods; ++p) {
+    if (!keep[p]) continue;
+    to[p] = kept++;
+    G_new = std::max<uint32_t>(G_new, std::max<uint32_t>((uint32_t)pods[p].slots.size(), pods[p].power_slots));
+  }
+  const uint32_t P_new = kept + kept / 4 + 64;
+  std::vector<uint32_t> src((size_t)P_new * G_new, GPR_ROW_NONE);
+  for (uint32_t p = 0; p < std::min(n_pods, P_old); ++p)
+    if (keep[p])
+      for (uint32_t g = 0; g < G_old; ++g) src[(size_t)to[p] * G_new + g] = p * G_old + g;
+  const auto t1 = std::chrono::steady_clock::now();
+  dev.resident_remap(P_new, G_new, src);
+  const double remap_ms = ms_since(t1);
+  asg.renumber_pods(to);
+  w.G = G_new, *pods_cap = P_new;
+  // the session's PROF rows equal this tick's (the delta check), so they belong to kept pods
+  for (auto& r : *prof_rows) r.first = to[r.first];
+  std::sort(prof_rows->begin(), prof_rows->end());
+  for (int k = 0; k < n_plans; ++k)
+    for (DevSeries& s : plans[k].series) s.pod = to[s.pod];
+  char line[200];
+  snprintf(line, sizeof line,
+           "Resident window reshaped on the GPU: %u -> %u, %u -> %u, %u pods dropped (live rows %.2f ms, remap %.2f ms)",
+           P_old, P_new, G_old, G_new, n_pods - kept, live_ms, remap_ms);
+  return line;
+}
+
 }  // namespace
 
 struct DeviceIngestSession::State {
@@ -450,8 +504,9 @@ Window DeviceIngestSession::ingest(const std::string& util, const std::string* p
     uint32_t g_now = 1;
     for (const PodEntry& pe : w.pods) g_now = std::max<uint32_t>(g_now, std::max<uint32_t>((uint32_t)pe.slots.size(), pe.power_slots));
     const char* why = nullptr;
-    if (w.pods.size() > st.pods_cap) why = "more pods than the resident window has rows for";
-    else if (g_now > w.G) why = "a pod gained a GPU slot beyond the resident window's shape";
+    const bool shape = w.pods.size() > st.pods_cap || g_now > w.G;  // what reshaping the ring can absorb
+    if (w.pods.size() > st.pods_cap && !opt.reshape) why = "more pods than the resident window has rows for";
+    else if (g_now > w.G && !opt.reshape) why = "a pod gained a GPU slot beyond the resident window's shape";
     // `A or B` (query.promql.j2:10-20) is resolved per tick at assignment time; if the set of PROF-fed rows
     // changes, UTIL samples that were (not) shadowed earlier in the window no longer match a fresh query
     else if (prof_rows != st.prof_rows) why = "the set of DCGM_FI_PROF_GR_ENGINE_ACTIVE series changed";
@@ -459,10 +514,18 @@ Window DeviceIngestSession::ingest(const std::string& util, const std::string* p
       st.valid = false;
       throw NeedFullWindow(why);
     }
-    w.P = (uint32_t)w.pods.size();
     w.t_end = opt.t_end;
     n_new = (uint32_t)(opt.slice_seconds / opt.step);
     dev_.resident_advance(n_new);
+    if (shape) {
+      try {
+        w.stats.ring_reshape = reshape_ring(dev_, w, asg, &st.pods_cap, &st.prof_rows, plans, n_plans);
+      } catch (const std::exception& e) {  // GPR_E_NOMEM included (the peak is the old ring plus the new one)
+        st.valid = false;
+        throw NeedFullWindow(std::string("the resident window could not be reshaped: ") + e.what());
+      }
+    }
+    w.P = (uint32_t)w.pods.size();
   }
   const bool resident = delta || opt.resident;
   const uint32_t n_rows = (resident ? st.pods_cap : w.P) * w.G;

@@ -67,6 +67,17 @@ class TextDevice {
     (void)pods, (void)G, (void)T, (void)with_power, (void)planes, (void)grid;
     throw std::logic_error("this device keeps no snapshots");
   }
+  // IngestOptions::reshape: the ring's rows moved to the shape [pods][G] (gpr_resident_remap: new row i holds old row
+  // src_rows[i], or no sample for GPR_ROW_NONE), and which rows hold a sample in either plane (gpr_resident_live_rows:
+  // bit r of (*bits)[r / 32]).  A device that cannot reshape throws; the session then takes the full range.
+  virtual void resident_remap(uint32_t pods, uint32_t G, const std::vector<uint32_t>& src_rows) {
+    (void)pods, (void)G, (void)src_rows;
+    throw std::logic_error("this device cannot reshape its ring");
+  }
+  virtual void resident_live_rows(std::vector<uint32_t>* bits) {
+    (void)bits;
+    throw std::logic_error("this device cannot reshape its ring");
+  }
 };
 
 struct DeviceIngestReport {

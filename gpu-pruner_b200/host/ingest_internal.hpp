@@ -224,6 +224,29 @@ class Assigner {
     power_keys_.resize(P);
     prof_sigs_ = std::move(prof_sigs);
   }
+  // Daemon mode, the resident ring reshaped (IngestOptions::reshape): pod p becomes pod to[p], in the same order, or
+  // leaves when to[p] == kDropped — with its power keys, its PROF signatures and the placed series that name it, so
+  // that a name that comes back is a new pod, as in a fresh ingest.  Skipped and Shadowed entries name no pod (their
+  // pod / slot are never read) and stay.
+  static constexpr uint32_t kDropped = 0xFFFFFFFFu;
+  void renumber_pods(const std::vector<uint32_t>& to) {
+    const PodList& old = w_.pods;
+    PodList kept;
+    std::vector<std::vector<uint64_t>> keys;
+    for (size_t p = 0; p < to.size(); ++p)
+      if (to[p] != kDropped) kept.push_back(old[p]), keys.push_back(power_keys_[p]);  // (one entry per pod)
+    std::map<std::pair<uint32_t, uint32_t>, std::vector<std::string>> sigs;
+    for (const auto& kv : prof_sigs_)
+      if (to[kv.first.first] != kDropped) sigs[std::make_pair(to[kv.first.first], kv.first.second)] = kv.second;
+    std::vector<Known> entries;
+    for (const Known& k : known_)
+      if ((k.h1 || k.h2) && (k.result != Placed || to[k.pod] != kDropped))
+        entries.push_back(Known{k.h1, k.h2, k.result, k.result == Placed ? to[k.pod] : k.pod, k.slot});
+    known_.clear(), n_known_ = 0;
+    for (const Known& k : entries) insert_known(k.h1, k.h2, k.result, k.pod, k.slot);
+    w_.pods = std::move(kept);
+    adopt_pods(std::move(keys), std::move(sigs));
+  }
 
   // Daemon mode: the same series comes back every tick and must keep its row.  A series is identified by the
   // bytes of its label map as the server prints them (sorted keys, so the text is canonical) plus the plane it

@@ -295,6 +295,18 @@ GPR_API int gpr_resident_head(gpr_ctx *ctx, uint32_t *head);
 #define GPR_ROW_NONE 0xFFFFFFFFu
 GPR_API int gpr_resident_remap(gpr_ctx *ctx, uint32_t n_pods, uint32_t n_gpus, const uint32_t *src_rows,
                                int32_t mem_kind);
+/* bit r of bits[r >> 5] (bit r & 31) = ring row r holds at least one sample in plane 0 or, if the ring has
+ * one, plane 1; ceil(n_rows / 32) words, padding bits zero.  host or device output (mem_kind).
+ * Every NaN cell counts as "no sample", not only the fill.  With GPR_F_BLOCK_INDEX and a current
+ * index the index rows are read instead of the planes (1/64 of the bytes); a stale index is not read
+ * and not refused.  Blocking, reads the ring only; decisions enqueued before it stay pending.  No
+ * resident window is GPR_E_STATE, a NULL bits or a bad mem_kind GPR_E_INVALID; on any error bits is
+ * untouched.
+ * The remap recipe of a daemon caller whose cluster outgrew the ring: open the tick's buckets
+ * (gpr_resident_advance), read the live rows, keep every pod with a live row or a series in the tick's
+ * slice, and gpr_resident_remap the kept pods' rows (and GPR_ROW_NONE for the new ones) into
+ * [kept + head-room][max(G, slots needed)]; then append the slice as on any tick.                    */
+GPR_API int gpr_resident_live_rows(gpr_ctx *ctx, uint32_t *bits, int32_t mem_kind);
 
 /* ---- multi-GPU: one process per GPU, pods sharded by rank, one allgather of the bitmap - */
 #define GPR_UNIQUE_ID_BYTES 128
