@@ -209,14 +209,20 @@ def split(ts, values, per_chunk=120):
     return [encode(ts[i:i + per_chunk], values[i:i + per_chunk]) for i in range(0, len(ts), per_chunk)]
 
 
-def encode_native(offsets, ts, bits, per_chunk=120):
-    """CSR samples (offsets u64, ts i64 ms, bits u64) -> (series_chunks, chunk_bytes, data) by the C++ encoder, built
-    with g++ into a temporary directory"""
+def build_native(d):
+    """the C++ encoder (tests/cpp/chunks_encode.cpp) built with g++ into directory d -> its path"""
     src = os.path.join(os.path.dirname(os.path.abspath(__file__)), "cpp", "chunks_encode.cpp")
+    exe = os.path.join(d, "chunks_encode")
+    subprocess.run(["g++", "-O2", "-std=c++17", "-Wall", "-Werror", src, "-o", exe], check=True,
+                   capture_output=True, text=True)
+    return exe
+
+
+def encode_native(offsets, ts, bits, per_chunk=120, exe=None):
+    """CSR samples (offsets u64, ts i64 ms, bits u64) -> (series_chunks, chunk_bytes, data) by the C++ encoder (`exe`
+    from build_native, or built with g++ into a temporary directory)"""
     with tempfile.TemporaryDirectory() as d:
-        exe = os.path.join(d, "chunks_encode")
-        subprocess.run(["g++", "-O2", "-std=c++17", "-Wall", "-Werror", src, "-o", exe], check=True,
-                       capture_output=True, text=True)
+        exe = exe or build_native(d)
         np.ascontiguousarray(offsets, np.uint64).tofile(os.path.join(d, "offsets.u64"))
         np.ascontiguousarray(ts, np.int64).tofile(os.path.join(d, "ts.i64"))
         np.ascontiguousarray(bits, np.uint64).tofile(os.path.join(d, "bits.u64"))

@@ -48,9 +48,9 @@ def export(plane, head, t_end, step, M):
     return sc, rows, cb, data, int(offsets[-1])
 
 
-def export_native(plane, head, t_end, step, M):
+def export_native(plane, head, t_end, step, M, exe=None):
     rows, offsets, ts, bits = flat(plane, head, t_end, step)
-    sc, cb, data = R.encode_native(offsets, ts, bits, M)
+    sc, cb, data = R.encode_native(offsets, ts, bits, M, exe)
     return sc, rows, cb, data, int(offsets[-1])
 
 
