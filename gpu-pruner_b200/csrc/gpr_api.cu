@@ -2244,13 +2244,26 @@ int gpr_chunks_scatter(gpr_ctx* ctx, const gpr_chunk_batch* batch, const gpr_tex
     return rc;
   if (bad) return chunk_batch_fault(ctx, bad, 0, grid->n_rows);
   if (host) {
+    constexpr uint32_t kBadIndex = gc::kBadChunkStart | gc::kBadChunkOrder;
     if (batch->chunk_bytes[0] != 0) bad |= gc::kBadChunkStart;
-    for (uint64_t c = 0; c < n_chunks && !bad; ++c) {
-      bad = gc::bound_faults(batch->chunk_bytes, c);
-      if (!bad && batch->chunk_bytes[c + 1] - batch->chunk_bytes[c] > gc::kHostPiece) bad = kChunkTooLarge;
-      if (bad) first = c;
+    for (uint64_t c = 0; c < n_chunks && !(bad & kBadIndex); ++c) {
+      uint32_t f = gc::bound_faults(batch->chunk_bytes, c);
+      if (!f && batch->chunk_bytes[c + 1] - batch->chunk_bytes[c] > gc::kHostPiece) f = kChunkTooLarge;
+      if (f && !bad) first = c;
+      bad |= f;
     }
-    if (bad) return chunk_batch_fault(ctx, bad, first, grid->n_rows);
+    if (bad) {
+      // Such a batch never goes up.  While chunk_bytes rises from 0 every chunk lies inside the data, so the chunks
+      // with good bounds are decoded here, as k_chunks_check decodes a device batch's: the first bad chunk and the
+      // faults are then those a device batch reports.
+      for (uint64_t c = 0; !(bad & kBadIndex) && batch->data && c < n_chunks; ++c) {
+        if (gc::bound_faults(batch->chunk_bytes, c)) continue;
+        const uint32_t f = gc::chunk_faults(batch->chunk_bytes, batch->data, 0, c);
+        bad |= f;
+        if (f && c < first) first = c;
+      }
+      return chunk_batch_fault(ctx, bad, first, grid->n_rows);
+    }
   }
   if (n_chunks && !batch->data) return fail(ctx, GPR_E_INVALID, "data is NULL");
   // the chunks' data, by the check kernel: in place for a device batch, piece by piece as it lands for a host one

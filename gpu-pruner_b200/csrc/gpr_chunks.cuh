@@ -111,7 +111,9 @@ GPR_HD uint64_t uvarint(Bits& r, bool* bad) {
 
 // ---- one chunk ---------------------------------------------------------------------------------------------------
 // Decodes the chunk [p, end) and calls emit(ts_ms, value) for each sample, in order; stops at the first fault.
-// Returns the fault bits (0 = the chunk is well formed).
+// Returns that fault's bit, as Prometheus' iterator reports its first error (0 = the chunk is well formed).  A bad
+// varint is found at its last byte, before the rest of its sample is read; a read past the end leaves every later
+// bit 0, so no window can be missing after it.
 template <typename Emit>
 GPR_HD uint32_t decode_chunk(const uint8_t* p, const uint8_t* end, Emit&& emit) {
   if (end - p < 2) return kShort;
@@ -156,7 +158,7 @@ GPR_HD uint32_t decode_chunk(const uint8_t* p, const uint8_t* end, Emit&& emit) 
     if (r.over || bad_varint) break;
     emit((int64_t)t, text::bits_to_double(v));
   }
-  return (r.over ? kOverrun : 0u) | (bad_varint ? kBadVarint : 0u) | (no_window ? kNoWindow : 0u);
+  return bad_varint ? kBadVarint : r.over ? kOverrun : no_window ? kNoWindow : 0u;
 }
 
 // What is wrong with chunk c's bounds: chunk_bytes[0] must be 0, and each chunk at least its 2-byte header.

@@ -16,7 +16,8 @@
 // DIR/series.u64 rows.u32 cbytes.u64 data.u8 plane.u32 (the plane before the call, n_rows x T)
 // DIR/out.bin: u32 fault bits (0 = accepted), u32 0, u64 first bad chunk (~0 if none), u64 n_in, u64 n_oow,
 // u64 n_tiny, then the plane after the call.  A rejected batch leaves the plane as it was.  The host walk of
-// chunk_faults and the check kernel must agree (exit 3).
+// chunk_faults and the check kernel must agree (exit 3).  A host batch whose chunk_bytes rises from 0 but has a chunk
+// with bad bounds is rejected by the host walk alone, which then decodes the other chunks as gpr_api.cu does.
 #include "cuda_shim.hpp"
 
 static inline unsigned long long atomicMin(unsigned long long* p, unsigned long long v) {
@@ -137,11 +138,15 @@ int main(int argc, char** argv) {
       host_bad |= f;
     }
     const bool bounds_ok = host_bad == 0;
-    if (bounds_ok) {
+    // chunk_bytes rises from 0 (every chunk inside the data): gpr_api.cu's host walk decodes the chunks whose own
+    // bounds are good, so a host batch then reports what a device batch does
+    const bool rising = !(host_bad & (gc::kBadChunkStart | gc::kBadChunkOrder));
+    if (rising) {
       if (data.size() != cbytes[n_chunks]) return 2;
       for (uint64_t c = 0; c < n_chunks; ++c) {
+        if (gc::bound_faults(cbytes.data(), c)) continue;
         const uint32_t f = gc::chunk_faults(cbytes.data(), data.data(), 0, c);
-        if (f && host_first == ~0ull) host_first = c;
+        if (f && c < host_first) host_first = c;
         host_bad |= f;
         if (!f) host_in += gc::chunk_count(data.data() + cbytes[c]);
       }
@@ -169,9 +174,9 @@ int main(int argc, char** argv) {
           return 0;
         });
       }
-      // bad bounds: the kernel also decodes the chunks whose own bounds are good, and may find more
-      const bool agree = bounds_ok ? k_bad == host_bad && (!host_bad || first == host_first)
-                                   : (k_bad & host_bad) == host_bad && first <= host_first;
+      // chunk_bytes not rising: the kernel also decodes the chunks whose own bounds are good, and may find more
+      const bool agree = rising ? k_bad == host_bad && (!host_bad || first == host_first)
+                                : (k_bad & host_bad) == host_bad && first <= host_first;
       if (!agree) {
         fprintf(stderr, "chunks: host check %u (chunk %llu) != kernel %u (chunk %llu)\n", host_bad, host_first, k_bad,
                 first);
