@@ -5,6 +5,7 @@
 #include "cli.hpp"
 
 #include <cerrno>
+#include <climits>
 #include <cstdlib>
 #include <functional>
 #include <map>
@@ -44,6 +45,7 @@ std::string usage() {
       "      --gpu-device <N>                       (extension) CUDA device ordinal [default: 0]\n"
       "      --snapshot-file <PATH>                 (extension) with -d: save the resident window after every tick, resume from it at start\n"
       "      --reshape-ring                         (extension) with -d: reshape the resident window on the GPU when pods or GPU slots outgrow it\n"
+      "      --query-slice <SECONDS>                (extension) ask ranges longer than this as consecutive queries of at most this length, merged on the GPU; no CPU-parser fallback for slices [default: 0 = one query]\n"
       "  -h, --help                                 Print help\n";
 }
 
@@ -140,6 +142,13 @@ ParseOutcome parse_cli(const std::vector<std::string>& args) {
   }};
   specs["snapshot-file"] = {0, true, [&](const std::string& v) { c.snapshot_file = v; return std::string(); }};
   specs["reshape-ring"] = {0, false, [&](const std::string&) { c.reshape_ring = true; return std::string(); }};
+  specs["query-slice"] = {0, true, [&](const std::string& v) {
+    uint64_t x = 0;
+    std::string e = parse_u64(v, &x);
+    if (e.empty() && x > (uint64_t)INT32_MAX) e = "number too large to fit in target type";
+    if (e.empty()) c.query_slice = (int64_t)x;
+    return e;
+  }};
   specs["now"] = {0, true, [&](const std::string& v) { return parse_i64(v, &c.now_override); }};
   specs["max-ticks"] = {0, true, [&](const std::string& v) {
     int64_t x;

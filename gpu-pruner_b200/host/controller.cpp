@@ -13,6 +13,8 @@
 #include <thread>
 #include <unordered_map>
 
+#include "ingest_device.hpp"
+
 namespace gph {
 
 // ---- logging (main.rs:157-243: default | json | pretty) --------------------------------------------
@@ -53,6 +55,27 @@ bool file_exists(const std::string& p) {
   return stat(p.c_str(), &st) == 0;
 }
 
+// a recorded response can be more than a gigabyte: one sized read, not a character iterator
+std::string read_file(const std::string& path, uint64_t* read_bytes) {
+  FILE* f = fopen(path.c_str(), "rb");
+  if (!f) throw std::runtime_error("cannot open " + path);
+  std::string s;
+  struct stat st;
+  if (fstat(fileno(f), &st) == 0 && st.st_size > 0) s.resize((size_t)st.st_size);
+  size_t got = 0;
+  while (got < s.size()) {
+    const size_t k = fread(&s[got], 1, s.size() - got, f);
+    if (k == 0) break;
+    got += k;
+  }
+  s.resize(got);
+  char tail[4096];  // a file that grew after fstat (or has no size): read on
+  for (size_t k; (k = fread(tail, 1, sizeof tail, f)) > 0;) s.append(tail, k);
+  fclose(f);
+  *read_bytes += s.size();
+  return s;
+}
+
 // file://DIR — recorded range-query responses instead of a Prometheus server:
 //   DIR/util.json [prof.json] [power.json] [dmi.json] [query.json = {"end": ts, "step": s}]     every tick the same
 //   DIR/tick-0000/..., DIR/tick-0001/...                                                       one directory per tick,
@@ -72,13 +95,17 @@ class FileSource : public WindowSource {
       if (!file_exists(base)) throw std::runtime_error("Failed to run query! " + base + " not found (no more recorded ticks)");
     }
     const bool can_reside = args.daemon_mode && ingestor_ != nullptr;
+    // --query-slice: a range longer than S seconds is asked as consecutive queries of at most S seconds
+    const int64_t S = ingestor_ ? args.query_slice : 0;
     // daemon mode with a resident window: ask only for what was scraped since the previous tick
     const int64_t since = can_reside ? ingestor_->resident_t_end() : 0;
-    if (since > 0 && file_exists(base + "/delta/util.json") && file_exists(base + "/delta/query.json")) {
+    const bool delta_there = file_exists(base + "/delta/util.json") || (S > 0 && file_exists(base + "/delta/slice-0000"));
+    if (since > 0 && delta_there && file_exists(base + "/delta/query.json")) {
       const Json meta = Json::parse_file(base + "/delta/query.json");
       const int64_t start = (int64_t)meta["start"].as_number(0), end = (int64_t)meta["end"].as_number(0);
       if (start == since && end > start) {
         try {
+          if (S > 0 && end - start > S) return load_slices(args, base + "/delta", start, end, S, true);
           return load(args, base + "/delta", end - start, true);
         } catch (const NeedFullWindow& e) {
           if (log_) log_->info(std::string("Resident window rebuilt from the full range: ") + e.what());
@@ -88,6 +115,12 @@ class FileSource : public WindowSource {
                    ", resident up to " + std::to_string(since) + "): using the full range");
       }
     }
+    if (S > 0 && args.duration * 60 > S) {
+      const std::string full = file_exists(base + "/full/query.json") ? base + "/full" : base;
+      const int64_t end = file_exists(full + "/query.json")
+                              ? (int64_t)Json::parse_file(full + "/query.json")["end"].as_number(0) : 0;
+      return load_slices(args, full, end - args.duration * 60, end, S, false);
+    }
     return load(args, file_exists(base + "/full/util.json") ? base + "/full" : base, 0, can_reside);
   }
 
@@ -95,28 +128,9 @@ class FileSource : public WindowSource {
   Window load(const Cli& args, const std::string& d, int64_t slice_seconds, bool resident) {
     const std::string up = d + "/util.json";
     if (!file_exists(up)) throw std::runtime_error("Failed to run query! " + up + " not found");
-    // a recorded response can be more than a gigabyte: one sized read, not a character iterator
     const auto read_t0 = std::chrono::steady_clock::now();
     uint64_t read_bytes = 0;
-    auto slurp = [&read_bytes](const std::string& path) {
-      FILE* f = fopen(path.c_str(), "rb");
-      if (!f) throw std::runtime_error("cannot open " + path);
-      std::string s;
-      struct stat st;
-      if (fstat(fileno(f), &st) == 0 && st.st_size > 0) s.resize((size_t)st.st_size);
-      size_t got = 0;
-      while (got < s.size()) {
-        const size_t k = fread(&s[got], 1, s.size() - got, f);
-        if (k == 0) break;
-        got += k;
-      }
-      s.resize(got);
-      char tail[4096];  // a file that grew after fstat (or has no size): read on
-      for (size_t k; (k = fread(tail, 1, sizeof tail, f)) > 0;) s.append(tail, k);
-      fclose(f);
-      read_bytes += s.size();
-      return s;
-    };
+    auto slurp = [&read_bytes](const std::string& path) { return read_file(path, &read_bytes); };
     const std::string util = slurp(up);
     std::string prof, power;
     const std::string *pprof = nullptr, *ppower = nullptr;
@@ -151,6 +165,66 @@ class FileSource : public WindowSource {
       if (log_ && !note.empty()) log_->info(note);
     }
     // node_type for the rows of PodMetricData: the node_dmi_info join of query.promql.j2:23-34
+    if (file_exists(d + "/dmi.json")) apply_node_types(w, Json::parse_file(d + "/dmi.json"));
+    return w;
+  }
+
+  // (start, end] asked as consecutive queries of at most S seconds, the newest ending at `end`: d/slice-0000/ (oldest)
+  // ... each with util.json [prof.json] [power.json] and query.json = {"start", "end", "step"} of that query.  A slice
+  // that is missing or answers another range fails the query; the session is cold then (ingest_slices reads the
+  // slices one by one, after it has given up the resident window).
+  Window load_slices(const Cli& args, const std::string& d, int64_t start, int64_t end, int64_t S, bool delta) {
+    if (!file_exists(d + "/query.json")) throw std::runtime_error("Failed to run query! " + d + "/query.json not found");
+    const int64_t step = (int64_t)Json::parse_file(d + "/query.json")["step"].as_number(0);
+    if (step <= 0 || S % step != 0)
+      throw std::runtime_error("Failed to run query! --query-slice " + std::to_string(S) +
+                               " s is not a whole number of the query step (" + std::to_string(step) +
+                               " s): slices would share buckets");
+    SlicedFetch f;
+    const int64_t n = (end - start + S - 1) / S;
+    for (int64_t j = 0; j < n; ++j) f.ranges.emplace_back(std::max(start, end - (n - j) * S), end - (n - 1 - j) * S);
+    auto dir = [&d](size_t j) {
+      char name[32];
+      snprintf(name, sizeof name, "/slice-%04zu", j);
+      return d + name;
+    };
+    const bool want_power = args.power_threshold && *args.power_threshold != 0.0;
+    f.has_prof = file_exists(dir(0) + "/prof.json");
+    f.has_power = want_power && file_exists(dir(0) + "/power.json");
+    uint64_t read_bytes = 0;
+    double read_ms = 0;
+    f.load = [&](int kind, size_t j, std::string* text) {
+      const auto t0 = std::chrono::steady_clock::now();
+      const std::string sd = dir(j);
+      if (!file_exists(sd + "/query.json")) throw std::runtime_error("Failed to run query! " + sd + "/query.json not found");
+      const Json q = Json::parse_file(sd + "/query.json");
+      const int64_t qs = (int64_t)q["start"].as_number(0), qe = (int64_t)q["end"].as_number(0);
+      if (qs != f.ranges[j].first || qe != f.ranges[j].second || (int64_t)q["step"].as_number(0) != step)
+        throw std::runtime_error("Failed to run query! recorded slice " + sd + " answers (" + std::to_string(qs) + ", " +
+                                 std::to_string(qe) + "], the query asks for (" + std::to_string(f.ranges[j].first) +
+                                 ", " + std::to_string(f.ranges[j].second) + "]");
+      static const char* const kFile[3] = {"/prof.json", "/util.json", "/power.json"};
+      const std::string path = sd + kFile[kind];
+      if (!file_exists(path)) throw std::runtime_error("Failed to run query! " + path + " not found");
+      *text = read_file(path, &read_bytes);
+      read_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    };
+    IngestOptions opt;
+    opt.duration_min = args.duration;
+    opt.power_threshold = want_power ? *args.power_threshold : 0.0;
+    opt.t_end = end, opt.step = step;
+    opt.slice_seconds = delta ? end - start : 0;
+    opt.resident = true;
+    opt.reshape = args.reshape_ring;
+    std::string note;
+    Window w = ingestor_->ingest_slices(args, f, opt, &note);
+    if (log_) {
+      char rbuf[200];
+      snprintf(rbuf, sizeof rbuf, "Recorded responses read from %s: %zu query slices of at most %lld s, %.1f MB in %.1f ms",
+               d.c_str(), f.ranges.size(), (long long)S, read_bytes / 1e6, read_ms);
+      log_->info(rbuf);
+      if (!note.empty()) log_->info(note);
+    }
     if (file_exists(d + "/dmi.json")) apply_node_types(w, Json::parse_file(d + "/dmi.json"));
     return w;
   }

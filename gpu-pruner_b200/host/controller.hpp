@@ -19,6 +19,7 @@
 namespace gph {
 
 class DeviceIngestSession;
+struct SlicedFetch;
 
 // lib.rs:136-145
 struct PodMetricData {
@@ -92,6 +93,12 @@ class TextIngestor {
   // daemon mode: newest second of the window this ingestor keeps resident between ticks (0 = none: the next
   // tick must bring the full range).  An ingest with opt.slice_seconds > 0 may throw NeedFullWindow.
   virtual int64_t resident_t_end() const { return 0; }
+  // --query-slice: the same range asked as several queries, merged into the resident window (ingest_device.hpp
+  // DeviceIngestSession::ingest_slices).  An ingestor without a resident window cannot take slices and throws.
+  virtual Window ingest_slices(const Cli& args, const SlicedFetch& f, const IngestOptions& opt, std::string* note) {
+    (void)args, (void)f, (void)opt, (void)note;
+    throw std::runtime_error("this ingestor cannot merge query slices");
+  }
   // daemon mode: the session that keeps the window resident, for snapshots (snapshot.hpp); created if need be.
   // nullptr (*error says why): this ingestor keeps no resident window, so there is nothing to snapshot.
   virtual DeviceIngestSession* resident_session(const Cli&, std::string* error) {

@@ -172,6 +172,29 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
     return w;
   }
 
+  Window ingest_slices(const Cli& args, const SlicedFetch& f, const IngestOptions& opt, std::string* note) override {
+    std::string error;
+    if (!ensure_ctx(args.gpu_device, &error)) throw std::runtime_error("Failed to run query! " + error);
+    const auto t0 = std::chrono::steady_clock::now();
+    DeviceIngestReport rep;
+    if (!session_) session_.reset(new DeviceIngestSession(*this));
+    Window w = session_->ingest_slices(f, opt, &rep);
+    const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    if (note) {
+      char buf[600];
+      snprintf(buf, sizeof buf,
+               "Device ingest: %llu series lists of %llu query slices over the last %lld s parsed on the GPU into the "
+               "resident %ux%ux%u window in %.1f ms (ring grown %llu times, %llu re-parsed on the CPU, %llu rows patched; "
+               "waiting for upload+scan %.1f, label maps (parallel) %.1f, rows (sequential) %.1f, parse %.1f ms)",
+               (unsigned long long)rep.spans, (unsigned long long)rep.slices,
+               (long long)(opt.slice_seconds > 0 ? opt.slice_seconds : w.span), w.P, w.G, w.T, ms,
+               (unsigned long long)rep.ring_growths, (unsigned long long)rep.hard_spans,
+               (unsigned long long)rep.rows_patched, rep.scan_ms, rep.labels_ms, rep.assign_ms, rep.parse_ms);
+      *note = buf;
+    }
+    return w;
+  }
+
  private:
   // ---- TextDevice over libgpr -------------------------------------------------------------------------
   void check(int rc, const char* what) {
@@ -201,6 +224,10 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
     check(gpr_text_parse(ctx_, slot, spans.data(), (uint32_t)spans.size(), &g, plane), "gpr_text_parse");
   }
   void patch_row(int plane, uint32_t row, uint32_t T, const float* data, uint32_t n_newest, bool resident) override {
+    patch_cols(plane, row, T, data, n_newest, 0, resident);
+  }
+  void patch_cols(int plane, uint32_t row, uint32_t T, const float* data, uint32_t n, uint32_t newer,
+                  bool resident) override {
     float *u = nullptr, *p = nullptr;
     uint32_t head = 0;  // dense planes: the newest bucket is column T - 1, as if the head were at 0
     if (resident) {
@@ -211,12 +238,13 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
       check(gpr_text_planes(ctx_, &u, &p), "gpr_text_planes");
     }
     float* base = (plane == 0 ? u : p) + (size_t)row * T;
-    // the newest n buckets sit at ring positions head - n .. head - 1 (mod T): at most two runs
-    const uint32_t first = (head + T - n_newest % T) % T;
-    const uint32_t run1 = std::min(n_newest, T - first);
+    // the n buckets ending `newer` before the newest sit at ring positions head - newer - n .. head - newer - 1
+    // (mod T): at most two runs
+    const uint32_t first = (head + 2 * T - newer % T - n % T) % T;
+    const uint32_t run1 = std::min(n, T - first);
     check(gpr_memcpy(ctx_, base + first, data, (size_t)run1 * sizeof(float), GPR_MEM_DEVICE, GPR_MEM_HOST), "row patch");
-    if (run1 < n_newest)
-      check(gpr_memcpy(ctx_, base, data + run1, (size_t)(n_newest - run1) * sizeof(float), GPR_MEM_DEVICE, GPR_MEM_HOST),
+    if (run1 < n)
+      check(gpr_memcpy(ctx_, base, data + run1, (size_t)(n - run1) * sizeof(float), GPR_MEM_DEVICE, GPR_MEM_HOST),
             "row patch");
   }
   void resident_init(uint32_t pods, uint32_t G, uint32_t T, bool with_power) override {

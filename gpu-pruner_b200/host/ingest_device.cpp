@@ -400,6 +400,94 @@ std::string reshape_ring(TextDevice& dev, Window& w, Assigner& asg, uint32_t* po
   return line;
 }
 
+// Parses the series of `texts` into plane `plane` (0 util, 1 power) on `grid` (its fill applies to the first text only),
+// then re-parses on the CPU every series feeding a row the device gave up on and writes back that row's buckets of
+// `patch`: a run of patch.T buckets ending at patch.t_end, `newer` buckets before the grid's newest one.
+void parse_plane(TextDevice& dev, Window& w, const std::vector<TextPlan*>& texts, int plane, TextDevice::TextGrid grid,
+                 const Window& patch, uint32_t newer, double power_threshold, DeviceIngestReport& rep) {
+  const uint32_t n_rows = grid.n_rows;
+  grid.power_threshold = plane == 1 ? power_threshold : 0.0;
+  std::vector<uint32_t> writers(n_rows, 0);
+  for (TextPlan* tp : texts)
+    for (const DevSeries& s : tp->series) ++writers[(size_t)s.pod * w.G + s.slot];
+  std::vector<std::vector<gpr_text_span>> spans(texts.size());
+  for (size_t k = 0; k < texts.size(); ++k) {
+    for (const DevSeries& s : texts[k]->series) {
+      gpr_text_span sp;
+      memset(&sp, 0, sizeof sp);
+      sp.begin = s.begin, sp.end = s.end, sp.row = s.pod * w.G + s.slot;
+      sp.flags = writers[sp.row] > 1 ? GPR_SPAN_SHARED : 0u;
+      spans[k].push_back(sp);
+    }
+    const auto tp = std::chrono::steady_clock::now();
+    dev.parse(texts[k]->slot, spans[k], grid, plane);
+    rep.parse_ms += ms_since(tp);
+    grid.fill = false;
+    rep.spans += spans[k].size();
+  }
+  // rows the device gave up on: re-parse every series feeding them with the CPU walker
+  std::vector<uint8_t> dirty(n_rows, 0);
+  bool any_dirty = false;
+  for (const auto& list : spans)
+    for (const gpr_text_span& sp : list)
+      if (sp.flags & GPR_SPAN_HARD) dirty[sp.row] = 1, any_dirty = true, ++rep.hard_spans;
+  std::vector<std::vector<float>> rows;
+  std::vector<uint32_t> row_ids;
+  std::vector<int64_t> row_slot(any_dirty ? n_rows : 0, -1);
+  const gpr::text::PowerSnap snap = gpr::text::power_snap(plane == 1 ? power_threshold : 0.0);
+  for (size_t k = 0; k < texts.size(); ++k) {
+    const std::string& t = *texts[k]->text;
+    for (const gpr_text_span& sp : spans[k]) {
+      if (!dirty[sp.row]) {
+        w.stats.samples_in += sp.n_in;
+        w.stats.samples_out_of_window += sp.n_oow;
+        w.stats.tiny_values_clamped += sp.n_tiny;
+        continue;
+      }
+      if (row_slot[sp.row] < 0) {
+        row_slot[sp.row] = (int64_t)rows.size();
+        rows.emplace_back(patch.T, std::numeric_limits<float>::quiet_NaN());
+        row_ids.push_back(sp.row);
+      }
+      float* row = rows[(size_t)row_slot[sp.row]].data();
+      for_each_sample(t.data() + sp.begin - 1, t.data() + sp.end + 1, [&](double ts, double v) {
+        ++w.stats.samples_in;
+        const int64_t col = column_of(patch, ts_millis(ts));
+        if (col < 0) {
+          ++w.stats.samples_out_of_window;
+          return;
+        }
+        merge_cell(row[col], to_cell(v, snap, &w.stats.tiny_values_clamped));
+      });
+    }
+  }
+  for (size_t i = 0; i < rows.size(); ++i)
+    dev.patch_cols(plane, row_ids[i], w.T, rows[i].data(), patch.T, newer, grid.resident);
+  rep.rows_patched += rows.size();
+}
+
+// The first failing check of a delta tick against the resident window (nullptr: the ring can take the tick): same
+// grid, contiguous with what is resident, the same power plane
+template <typename State>
+const char* delta_blocker(const State& st, const IngestOptions& opt, bool with_power) {
+  if (!st.valid) return "nothing resident";
+  if (opt.step != st.w.step || opt.duration_min * 60 != st.w.span) return "step / window length changed";
+  if (opt.t_end - opt.slice_seconds != st.w.t_end) return "the slice does not start where the resident window ends";
+  if (opt.slice_seconds % opt.step != 0) return "the slice is not a whole number of steps";
+  if (opt.slice_seconds / opt.step >= (int64_t)st.w.T) return "the slice is as long as the window";
+  if (with_power != st.with_power) return "power plane appeared / disappeared";
+  if (with_power && !(opt.power_threshold == st.power_threshold ||
+                      (std::isnan(opt.power_threshold) && std::isnan(st.power_threshold))))
+    return "the power threshold changed";
+  return nullptr;
+}
+
+uint32_t slots_needed(const Window& w) {
+  uint32_t g = 1;
+  for (const PodEntry& pe : w.pods) g = std::max<uint32_t>(g, std::max<uint32_t>((uint32_t)pe.slots.size(), pe.power_slots));
+  return g;
+}
+
 }  // namespace
 
 struct DeviceIngestSession::State {
@@ -436,17 +524,7 @@ Window DeviceIngestSession::ingest(const std::string& util, const std::string* p
 
   if (delta) {
     // what must hold for the ring to take this tick: same grid, contiguous with what is resident
-    const char* why = nullptr;
-    if (!st.valid) why = "nothing resident";
-    else if (opt.step != st.w.step || opt.duration_min * 60 != st.w.span) why = "step / window length changed";
-    else if (opt.t_end - opt.slice_seconds != st.w.t_end) why = "the slice does not start where the resident window ends";
-    else if (opt.slice_seconds % opt.step != 0) why = "the slice is not a whole number of steps";
-    else if (opt.slice_seconds / opt.step >= (int64_t)st.w.T) why = "the slice is as long as the window";
-    else if ((power != nullptr) != st.with_power) why = "power plane appeared / disappeared";
-    else if (power && !(opt.power_threshold == st.power_threshold ||
-                        (std::isnan(opt.power_threshold) && std::isnan(st.power_threshold))))
-      why = "the power threshold changed";
-    if (why) {
+    if (const char* why = delta_blocker(st, opt, power != nullptr)) {
       st.valid = false;
       throw NeedFullWindow(why);
     }
@@ -540,85 +618,145 @@ Window DeviceIngestSession::ingest(const std::string& util, const std::string* p
     return result();
   }
 
-  // window the parse accepts: the whole range, or only the tick's slice
-  const int64_t parse_span = delta ? opt.slice_seconds : w.span;
-  const uint32_t patch_cols = delta ? n_new : w.T;
-  auto run_plane = [&](std::vector<TextPlan*> texts, int plane) {
-    std::vector<uint32_t> writers(n_rows, 0);
-    for (TextPlan* tp : texts)
-      for (const DevSeries& s : tp->series) ++writers[(size_t)s.pod * w.G + s.slot];
-    std::vector<std::vector<gpr_text_span>> spans(texts.size());
-    bool fill = !resident;
-    for (size_t k = 0; k < texts.size(); ++k) {
-      for (const DevSeries& s : texts[k]->series) {
-        gpr_text_span sp;
-        memset(&sp, 0, sizeof sp);
-        sp.begin = s.begin, sp.end = s.end, sp.row = s.pod * w.G + s.slot;
-        sp.flags = writers[sp.row] > 1 ? GPR_SPAN_SHARED : 0u;
-        spans[k].push_back(sp);
-      }
-      const auto tp = std::chrono::steady_clock::now();
-      TextDevice::TextGrid grid;
-      grid.t_end = w.t_end, grid.span = parse_span, grid.step = w.step, grid.T = w.T, grid.n_rows = n_rows;
-      grid.fill = fill, grid.resident = resident;
-      grid.power_threshold = plane == 1 ? opt.power_threshold : 0.0;
-      dev_.parse(texts[k]->slot, spans[k], grid, plane);
-      rep.parse_ms += ms_since(tp);
-      fill = false;
-      rep.spans += spans[k].size();
-    }
-    // rows the device gave up on: re-parse every series feeding them with the CPU walker
-    std::vector<uint8_t> dirty(n_rows, 0);
-    bool any_dirty = false;
-    for (const auto& list : spans)
-      for (const gpr_text_span& sp : list)
-        if (sp.flags & GPR_SPAN_HARD) dirty[sp.row] = 1, any_dirty = true, ++rep.hard_spans;
-    std::vector<std::vector<float>> rows;
-    std::vector<uint32_t> row_ids;
-    std::vector<int64_t> row_slot(any_dirty ? n_rows : 0, -1);
-    Window bucket;  // the grid of the patched columns: the newest `patch_cols` buckets
-    bucket.t_end = w.t_end, bucket.step = w.step, bucket.span = parse_span, bucket.T = patch_cols;
-    const gpr::text::PowerSnap snap = gpr::text::power_snap(plane == 1 ? opt.power_threshold : 0.0);
-    for (size_t k = 0; k < texts.size(); ++k) {
-      const std::string& t = *texts[k]->text;
-      for (const gpr_text_span& sp : spans[k]) {
-        if (!dirty[sp.row]) {
-          w.stats.samples_in += sp.n_in;
-          w.stats.samples_out_of_window += sp.n_oow;
-          w.stats.tiny_values_clamped += sp.n_tiny;
-          continue;
-        }
-        if (row_slot[sp.row] < 0) {
-          row_slot[sp.row] = (int64_t)rows.size();
-          rows.emplace_back(patch_cols, std::numeric_limits<float>::quiet_NaN());
-          row_ids.push_back(sp.row);
-        }
-        float* row = rows[(size_t)row_slot[sp.row]].data();
-        for_each_sample(t.data() + sp.begin - 1, t.data() + sp.end + 1, [&](double ts, double v) {
-          ++w.stats.samples_in;
-          const int64_t col = column_of(bucket, ts_millis(ts));
-          if (col < 0) {
-            ++w.stats.samples_out_of_window;
-            return;
-          }
-          merge_cell(row[col], to_cell(v, snap, &w.stats.tiny_values_clamped));
-        });
-      }
-    }
-    for (size_t i = 0; i < rows.size(); ++i) dev_.patch_row(plane, row_ids[i], w.T, rows[i].data(), patch_cols, resident);
-    rep.rows_patched += rows.size();
-  };
+  // window the parse accepts: the whole range, or only the tick's slice; the CPU re-parse patches the same buckets
+  TextDevice::TextGrid grid;
+  grid.t_end = w.t_end, grid.span = delta ? opt.slice_seconds : w.span, grid.step = w.step, grid.T = w.T;
+  grid.n_rows = n_rows, grid.fill = !resident, grid.resident = resident;
+  Window patch;
+  patch.t_end = w.t_end, patch.step = w.step, patch.span = grid.span, patch.T = delta ? n_new : w.T;
   std::vector<TextPlan*> util_texts;
   if (pl_prof) util_texts.push_back(pl_prof);
   util_texts.push_back(pl_util);
-  run_plane(util_texts, 0);
-  if (pl_power) run_plane({pl_power}, 1);
+  parse_plane(dev_, w, util_texts, 0, grid, patch, 0, opt.power_threshold, rep);
+  if (pl_power) parse_plane(dev_, w, {pl_power}, 1, grid, patch, 0, opt.power_threshold, rep);
   rep.on_device = true;
   Window out = result();
   if (!resident) {
     out.d_util = dev_.plane(0);
     if (pl_power) out.d_power = dev_.plane(1);
   }
+  return out;
+}
+
+// A range asked as several queries (--query-slice, DESIGN.md §8e).  Every slice is planned and parsed before the next
+// one is read: PROF slices first, then UTIL, then POWER, each oldest first — so every PROF series of the range is known
+// before a UTIL series is assigned, and `A or B` shadows exactly as in one query.  Each slice is parsed against the
+// grid of the whole fetch; slices meet on the bucket grid, so a row the device declines is patched in its slice's
+// buckets only.  The session is valid again only after the last slice.
+Window DeviceIngestSession::ingest_slices(const SlicedFetch& f, const IngestOptions& opt, DeviceIngestReport* report) {
+  DeviceIngestReport local;
+  DeviceIngestReport& rep = report ? *report : local;
+  rep = DeviceIngestReport{};
+  State& st = *st_;
+  const bool delta = opt.slice_seconds > 0;
+  if (delta) {
+    if (const char* why = delta_blocker(st, opt, f.has_power)) {
+      st.valid = false;
+      throw NeedFullWindow(why);
+    }
+  }
+  st.valid = false;
+  if (opt.t_end <= 0 || opt.step <= 0) throw std::runtime_error("a sliced query needs the window end and step (query.json)");
+  const int64_t span = delta ? opt.slice_seconds : std::max<int64_t>(1, opt.duration_min * 60);
+  // the slices must tile (t_end - span, t_end] and meet on the bucket grid
+  if (f.ranges.empty() || f.ranges.front().first != opt.t_end - span || f.ranges.back().second != opt.t_end)
+    throw std::runtime_error("the query slices do not cover the queried range");
+  for (size_t j = 0; j < f.ranges.size(); ++j)
+    if (f.ranges[j].first >= f.ranges[j].second || (j && f.ranges[j].first != f.ranges[j - 1].second) ||
+        (opt.t_end - f.ranges[j].second) % opt.step != 0)
+      throw std::runtime_error("query slice " + std::to_string(j) + " does not meet its neighbours on the bucket grid");
+  if (!delta) {
+    st.w = Window();
+    st.asg.reset(new Assigner(st.w));
+    st.prof_rows.clear();
+    st.pods_cap = 0;
+    st.with_power = f.has_power;
+    st.power_threshold = opt.power_threshold;
+    finish_shape(st.w, opt, 0, 1, f.has_power, /*allocate=*/false);  // the grid; the shape follows the slices
+  }
+  Window& w = st.w;
+  w.stats = IngestStats();
+  Assigner& asg = *st.asg;
+  if (delta) {
+    w.t_end = opt.t_end;
+    dev_.resident_advance((uint32_t)(opt.slice_seconds / opt.step));
+  }
+  // the ring keeps every row it has; new pods and slots get rows of their own
+  auto grow = [&](uint32_t pods, uint32_t G) {
+    std::vector<uint32_t> src((size_t)pods * G, GPR_ROW_NONE);
+    for (uint32_t p = 0; p < std::min(pods, st.pods_cap); ++p)
+      for (uint32_t g = 0; g < w.G; ++g) src[(size_t)p * G + g] = p * w.G + g;
+    try {
+      dev_.resident_remap(pods, G, src);
+    } catch (const std::exception& e) {
+      if (delta) throw NeedFullWindow(std::string("the resident window could not be grown: ") + e.what());
+      throw;
+    }
+    st.pods_cap = pods, w.G = G;
+  };
+  TextDevice::TextGrid grid;
+  grid.t_end = w.t_end, grid.span = span, grid.step = w.step, grid.T = w.T;
+  grid.fill = false, grid.resident = true;
+  std::vector<std::pair<uint32_t, uint32_t>> prof_rows;
+  for (int kind = 0; kind < 3; ++kind) {  // 0 PROF, 1 UTIL, 2 POWER: the order the one-query paths assign rows in
+    if (kind == 1) {
+      std::sort(prof_rows.begin(), prof_rows.end());  // the union: a series in several slices feeds one row
+      prof_rows.erase(std::unique(prof_rows.begin(), prof_rows.end()), prof_rows.end());
+      // `A or B` over the whole window: the PROF-fed rows of every slice against those of the resident window
+      if (delta && prof_rows != st.prof_rows) throw NeedFullWindow("the set of DCGM_FI_PROF_GR_ENGINE_ACTIVE series changed");
+    }
+    if ((kind == 0 && !f.has_prof) || (kind == 2 && !f.has_power)) continue;
+    for (size_t j = 0; j < f.ranges.size(); ++j) {
+      std::string text;
+      f.load(kind, j, &text);
+      TextPlan plan;
+      plan.slot = kind, plan.text = &text;
+      try {
+        plan_text(dev_, plan, asg, w, kind == 2, kind == 0, rep, /*remember=*/true);
+      } catch (const NotCompact& e) {
+        const std::string why = "device ingest not possible for query slice " + std::to_string(j) + ": " + e.why;
+        if (delta) throw NeedFullWindow(why);
+        throw std::runtime_error(why);
+      } catch (const DeviceDeclined& e) {
+        const std::string why = "device ingest not possible for query slice " + std::to_string(j) + ": " + e.what();
+        if (delta) throw NeedFullWindow(why);
+        throw std::runtime_error(why);
+      }
+      if (kind == 0)
+        for (const DevSeries& s : plan.series) prof_rows.emplace_back(s.pod, s.slot);
+      const uint32_t n_pods = (uint32_t)w.pods.size(), g_now = slots_needed(w);
+      if (st.pods_cap == 0) {  // the first slice of a full fetch: the ring, with the usual head-room
+        st.pods_cap = n_pods + n_pods / 4 + 64, w.G = g_now;
+        dev_.resident_init(st.pods_cap, w.G, w.T, st.with_power);
+      } else if (n_pods > st.pods_cap || g_now > w.G) {
+        if (delta && !opt.reshape)
+          throw NeedFullWindow(n_pods > st.pods_cap ? "more pods than the resident window has rows for"
+                                                    : "a pod gained a GPU slot beyond the resident window's shape");
+        grow(std::max(st.pods_cap, n_pods + n_pods / 4 + 64), std::max(w.G, g_now));
+        ++rep.ring_growths;
+      }
+      // this slice's buckets: (ranges[j].first, ranges[j].second], `newer` buckets before the newest of the grid
+      Window patch;
+      patch.t_end = f.ranges[j].second, patch.step = w.step, patch.span = f.ranges[j].second - f.ranges[j].first;
+      const uint32_t newer = (uint32_t)((w.t_end - patch.t_end) / w.step);
+      patch.T = (uint32_t)std::min<int64_t>(w.T - newer, (patch.span + w.step - 1) / w.step);
+      grid.n_rows = st.pods_cap * w.G;
+      parse_plane(dev_, w, {&plan}, kind == 2 ? 1 : 0, grid, patch, newer, opt.power_threshold, rep);
+    }
+  }
+  if (!delta) {
+    st.prof_rows = prof_rows;
+    // the shape a one-query ingest of the range gives the ring, so that later ticks take the same path
+    const uint32_t n_pods = (uint32_t)w.pods.size(), want = n_pods + n_pods / 4 + 64, g_now = slots_needed(w);
+    if (want != st.pods_cap || g_now != w.G) grow(want, g_now), ++rep.ring_growths;
+  }
+  w.P = (uint32_t)w.pods.size();
+  rep.on_device = true;
+  rep.slices = f.ranges.size();
+  Window out = w;
+  out.resident = true;
+  out.resident_pods = st.pods_cap, out.resident_power = st.with_power;
+  st.valid = true;
   return out;
 }
 

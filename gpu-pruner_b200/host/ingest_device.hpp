@@ -6,6 +6,7 @@
 // cell for cell (tests/test_text_device_cpu.py on an emulated device, tests/test_gpu_text.py on the GPU).
 #pragma once
 #include <cstdint>
+#include <functional>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -47,6 +48,13 @@ class TextDevice {
   // overwrite the newest `n_newest` buckets of `row` (chronological order in `data`; n_newest == T: the whole
   // row) — rows the strict device parser declined, re-parsed on the CPU
   virtual void patch_row(int plane, uint32_t row, uint32_t T, const float* data, uint32_t n_newest, bool resident) = 0;
+  // patch_row for any run of buckets: the `n` buckets that end `newer` buckets before the newest (a slice of a range
+  // asked as several queries).  A device that patches only the newest buckets throws for newer > 0.
+  virtual void patch_cols(int plane, uint32_t row, uint32_t T, const float* data, uint32_t n, uint32_t newer,
+                          bool resident) {
+    if (newer) throw std::logic_error("this device patches only the newest buckets of a row");
+    patch_row(plane, row, T, data, n, resident);
+  }
   virtual const float* plane(int plane) = 0;
   // daemon mode: (re)create the resident ring [rows][T] (all "no sample"), and open the next n_new buckets
   virtual void resident_init(uint32_t pods, uint32_t G, uint32_t T, bool with_power) = 0;
@@ -84,6 +92,7 @@ struct DeviceIngestReport {
   bool on_device = false;        // false: the CPU text path produced the window (reason says why)
   std::string reason;
   uint64_t spans = 0, hard_spans = 0, rows_patched = 0;
+  uint64_t slices = 0, ring_growths = 0;  // ingest_slices: queries per metric, and how often the ring grew on the way
   // where the time went: device scan (text upload + marker scan), series walk over the markers,
   // label maps -> rows, device parse (NaN fill + sample parse)
   double scan_ms = 0, labels_ms = 0, assign_ms = 0, parse_ms = 0;
@@ -96,6 +105,15 @@ Window ingest_matrix_device(TextDevice& dev, const std::string& util, const std:
                             const std::string* power, const IngestOptions& opt,
                             DeviceIngestReport* report = nullptr);
 
+// A range asked as consecutive queries (--query-slice): slice j covers (ranges[j].first, ranges[j].second], oldest
+// first, each starting where the previous one ends.  load(kind, j, &text) reads the response of metric `kind` (0 PROF,
+// 1 UTIL, 2 POWER) for slice j, or throws; it is called only for the metrics the fetch has.
+struct SlicedFetch {
+  std::vector<std::pair<int64_t, int64_t>> ranges;
+  bool has_prof = false, has_power = false;
+  std::function<void(int kind, size_t j, std::string* text)> load;
+};
+
 // Daemon mode (main.rs:286-330): the row assignment and the window survive between ticks.  The first tick (and
 // any tick after NeedFullWindow) ingests the full range query into the engine's resident ring; later ticks ingest
 // only what was scraped since (opt.slice_seconds), appended to the ring.  Pods and slots keep their rows for the
@@ -107,6 +125,13 @@ class DeviceIngestSession {
   // opt.slice_seconds == 0: full window (re)build; > 0: delta — throws NeedFullWindow if it cannot be absorbed
   Window ingest(const std::string& util, const std::string* prof, const std::string* power, const IngestOptions& opt,
                 DeviceIngestReport* report = nullptr);
+  // The same fetch asked as several queries (--query-slice, DESIGN.md §8e): full (opt.slice_seconds == 0) or delta, into
+  // the resident ring, with the result a one-query ingest of the range gives.  The ring starts from the first slice and
+  // grows (gpr_resident_remap, nothing dropped) when a later slice brings more pods or slots; a full fetch ends with the
+  // one-query shape [P + P/4 + 64][G].  A delta that outgrows the ring throws NeedFullWindow as ingest() does, unless
+  // opt.reshape.  Throws std::runtime_error for a slice that fails or a response the device cannot take (no CPU
+  // fallback here); the session then stays cold.
+  Window ingest_slices(const SlicedFetch& f, const IngestOptions& opt, DeviceIngestReport* report = nullptr);
   // newest second the resident window holds (0 = nothing resident): the next delta must start right after it
   int64_t resident_t_end() const;
   void invalidate();

@@ -40,8 +40,14 @@ int main(int argc, char** argv) {
   std::unique_ptr<gph::TextIngestor> cpu_ingestor;
   gph::TextIngestor* ingestor = engine->text_ingestor();
   if (ing && std::string(ing) == "cpu") cpu_ingestor = gph::make_cpu_text_ingestor(), ingestor = cpu_ingestor.get();
+  // --query-slice merges the slices into the resident window on the GPU; the CPU ingest asks for whole ranges
+  gph::Cli run = cli;
+  if (cpu_ingestor && run.query_slice > 0) {
+    log.warn("--query-slice ignored: slicing needs the device ingest (GPR_INGEST=cpu asks for whole ranges)");
+    run.query_slice = 0;
+  }
   std::unique_ptr<gph::WindowSource> src = gph::make_window_source(cli.prometheus_url, ingestor, &log);
-  gph::Controller ctl(cli, kube.get(), engine.get(), log, gph::system_clock());
+  gph::Controller ctl(run, kube.get(), engine.get(), log, gph::system_clock());
   // --snapshot-file: the resident window survives a restart (snapshot.hpp).  The CPU ingest keeps no resident window,
   // so there is nothing to save: said once, and the run is the one without the flag.
   std::unique_ptr<gph::WindowSnapshots> snapshots;
