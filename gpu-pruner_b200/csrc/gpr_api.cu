@@ -241,6 +241,7 @@ struct gpr_ctx {
   Buf<uint32_t> d_remap_map;            // a host map, uploaded
   Buf<unsigned int> d_remap_check;      // a device map's check: [first bad new row | seen bitmap | dup bitmap]
   Buf<uint32_t> d_live;                 // gpr_resident_live_rows' bitmap for a host destination
+  Buf<uint32_t> d_band;                 // gpr_resident_cols' band for a host destination
 
   // device-side ingest of response text (gpr_text_scan / gpr_text_parse)
   Buf<uint8_t> d_text[3];
@@ -1515,6 +1516,38 @@ int gpr_resident_live_rows(gpr_ctx* ctx, uint32_t* bits, int32_t mem_kind) {
   if (rc != GPR_OK) return rc;
   if (mem_kind == GPR_MEM_HOST)
     CU(cudaMemcpyAsync(bits, out, (size_t)words * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return GPR_OK;
+  GPR_CATCH(ctx)
+}
+
+int gpr_resident_cols(gpr_ctx* ctx, int32_t plane, uint32_t newer, uint32_t n_cols, float* out, int32_t mem_kind) {
+  if (!ctx) return GPR_E_INVALID;
+  GPR_TRY
+  NvtxRange nvtx_range("gpr_resident_cols");
+  if (const int rc = enter(ctx)) return rc;
+  if (!ctx->d_res_util) return fail(ctx, GPR_E_STATE, "no resident window (gpr_resident_init)");
+  if (plane != 0 && plane != 1) return fail(ctx, GPR_E_INVALID, "bad plane %d", plane);
+  if (plane == 1 && !ctx->d_res_power) return fail(ctx, GPR_E_STATE, "the resident window has no power plane");
+  if (n_cols == 0) return fail(ctx, GPR_E_INVALID, "n_cols is 0");
+  if ((uint64_t)newer + n_cols > ctx->res_T)
+    return fail(ctx, GPR_E_INVALID, "newer + n_cols = %llu > n_samples = %u", (unsigned long long)newer + n_cols,
+                ctx->res_T);
+  if (!out) return fail(ctx, GPR_E_INVALID, "out is NULL");
+  if (mem_kind != GPR_MEM_HOST && mem_kind != GPR_MEM_DEVICE) return fail(ctx, GPR_E_INVALID, "bad mem_kind %d", mem_kind);
+  const size_t rows = (size_t)ctx->res_P * ctx->res_G, cells = rows * n_cols;
+  uint32_t* dst = reinterpret_cast<uint32_t*>(out);
+  if (mem_kind == GPR_MEM_HOST) {
+    CU(ctx->d_band.grow(ctx->stream, cells));
+    dst = ctx->d_band;
+  }
+  const float* src = plane == 0 ? ctx->d_res_util : ctx->d_res_power;
+  const int rc = launch(ctx, gpr::k_ring_cols, gpr::ring_grid(rows, ctx->sm_count), gpr::kRingThreads, 0, false, dst,
+                        reinterpret_cast<const uint32_t*>(src), (uint32_t)rows, ctx->res_T,
+                        gpr::ring_cols_start(ctx->res_head, ctx->res_T, newer, n_cols), n_cols);
+  if (rc != GPR_OK) return rc;
+  if (mem_kind == GPR_MEM_HOST)
+    CU(cudaMemcpyAsync(out, dst, cells * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   return GPR_OK;
   GPR_CATCH(ctx)

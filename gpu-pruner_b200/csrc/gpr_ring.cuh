@@ -5,7 +5,8 @@
 // gpr_resident_advance (which source columns survive, where they land, what each plane gets, the grid, the index
 // row length) is plain functions.  gpr_api.cu launches what these return; tests/cpp/ring_emul.cpp runs the same
 // source on the CPU against a numpy model of the ring.  gpr_resident_remap's row gather and map check are here too
-// (tests/cpp/remap_emul.cpp), and gpr_resident_live_rows' row test (tests/cpp/live_rows_emul.cpp).
+// (tests/cpp/remap_emul.cpp), gpr_resident_live_rows' row test (tests/cpp/live_rows_emul.cpp) and gpr_resident_cols'
+// band gather (tests/cpp/ring_cols_emul.cpp).
 #pragma once
 
 #include <stddef.h>
@@ -284,6 +285,29 @@ __global__ void __launch_bounds__(kRingThreads) k_live_rows(const uint32_t* __re
     }
     const uint32_t word = __ballot_sync(0xFFFFFFFFu, mine);
     if (lane == 0) bits[w] = word;
+  }
+}
+
+// ---- gpr_resident_cols: a band of the ring's newest buckets, read out oldest first
+// Ring position of the band's oldest bucket: the n_cols buckets that end `newer` buckets before the newest, which is at
+// (head + T - 1) % T.  Needs newer + n_cols <= T.
+inline uint32_t ring_cols_start(uint32_t head, uint32_t T, uint32_t newer, uint32_t n_cols) {
+  return (uint32_t)(((uint64_t)head + T - newer - n_cols) % T);
+}
+
+// out[r * n_cols + j] = ring row r at position (start + j) % T: one row per CTA and round (grid: ring_grid), the band
+// gathered across the ring's wrap point.  Words are moved as bits, so every NaN payload comes out as it is stored.
+__global__ void __launch_bounds__(kRingThreads) k_ring_cols(uint32_t* __restrict__ out,
+                                                            const uint32_t* __restrict__ plane, uint32_t n_rows,
+                                                            uint32_t T, uint32_t start, uint32_t n_cols) {
+  for (uint32_t r = blockIdx.x; r < n_rows; r += gridDim.x) {
+    const uint32_t* in = plane + (size_t)r * T;
+    uint32_t* o = out + (size_t)r * n_cols;
+    for (uint32_t j = threadIdx.x; j < n_cols; j += blockDim.x) {
+      uint32_t t = start + j;
+      if (t >= T) t -= T;
+      o[j] = in[t];
+    }
   }
 }
 

@@ -577,6 +577,18 @@ class IdleEngine:
         self._check(self._lib.gpr_resident_live_rows(self._h, words.ctypes.data, ffi.GPR_MEM_HOST))
         return np.unpackbits(words.view(np.uint8), bitorder="little")[:rows].astype(bool)
 
+    def resident_cols(self, plane: int, newer: int, n_cols: int) -> np.ndarray:
+        """A band of the resident ring (gpr_resident_cols): the ``n_cols`` buckets that end ``newer`` buckets before
+        the newest, oldest first, of plane ``plane`` (0 util, 1 power) for every row — a float32 array
+        ``[P * G, n_cols]``, row ``pod * G + slot``, NaN where a bucket holds no sample."""
+        rows = getattr(self, "_res_rows", None)
+        if rows is None:
+            raise RuntimeError("no resident window (resident_init)")
+        out = np.empty((rows, max(0, int(n_cols))), np.float32)
+        self._check(self._lib.gpr_resident_cols(self._h, int(plane), int(newer), int(n_cols), out.ctypes.data,
+                                                ffi.GPR_MEM_HOST))
+        return out
+
     def text_planes(self):
         u, w = C.c_void_p(), C.c_void_p()
         self._check(self._lib.gpr_text_planes(self._h, C.byref(u), C.byref(w)))

@@ -46,6 +46,7 @@ std::string usage() {
       "      --snapshot-file <PATH>                 (extension) with -d: save the resident window after every tick, resume from it at start\n"
       "      --reshape-ring                         (extension) with -d: reshape the resident window on the GPU when pods or GPU slots outgrow it\n"
       "      --query-slice <SECONDS>                (extension) ask ranges longer than this as consecutive queries of at most this length, merged on the GPU; no CPU-parser fallback for slices [default: 0 = one query]\n"
+      "      --late-seconds <SECONDS>               (extension) with -d: ask every tick again for the newest SECONDS of the resident window, so samples that reach Prometheus late still count [default: 0 = off]\n"
       "  -h, --help                                 Print help\n";
 }
 
@@ -149,6 +150,14 @@ ParseOutcome parse_cli(const std::vector<std::string>& args) {
     if (e.empty()) c.query_slice = (int64_t)x;
     return e;
   }};
+  bool late_given = false;
+  specs["late-seconds"] = {0, true, [&](const std::string& v) {
+    uint64_t x = 0;
+    std::string e = parse_u64(v, &x);
+    if (e.empty() && x > (uint64_t)INT32_MAX) e = "number too large to fit in target type";
+    if (e.empty()) c.late_seconds = (int64_t)x, late_given = true;
+    return e;
+  }};
   specs["now"] = {0, true, [&](const std::string& v) { return parse_i64(v, &c.now_override); }};
   specs["max-ticks"] = {0, true, [&](const std::string& v) {
     int64_t x;
@@ -215,6 +224,12 @@ ParseOutcome parse_cli(const std::vector<std::string>& args) {
     return fail("the argument '--snapshot-file <PATH>' can only be used with '--daemon-mode'");
   if (c.reshape_ring && !c.daemon_mode)
     return fail("the argument '--reshape-ring' can only be used with '--daemon-mode'");
+  if (late_given && !c.daemon_mode)
+    return fail("the argument '--late-seconds <SECONDS>' can only be used with '--daemon-mode'");
+  if (c.late_seconds > 0 && c.late_seconds >= c.duration * 60)
+    return fail("invalid value '" + std::to_string(c.late_seconds) + "' for '--late-seconds <SECONDS>': must be less " +
+                "than the window (--duration " + std::to_string(c.duration) + " = " + std::to_string(c.duration * 60) +
+                " s)");
   if (!have_url && !c.print_query)
     return fail("the following required arguments were not provided:\n  --prometheus-url <PROMETHEUS_URL>");
   out.ok = true;

@@ -45,6 +45,9 @@ struct Cli {
   int64_t query_slice = 0;                    // --query-slice SECONDS: a range longer than this is asked as consecutive
                                               // queries of at most this length, merged into the resident window on the
                                               // GPU (DESIGN.md §8e); 0 = one query per range
+  int64_t late_seconds = 0;                   // --late-seconds L (-d only): every delta tick asks again for the newest L
+                                              // seconds of the resident window, so samples that reach the server up to
+                                              // L s late still count (DESIGN.md §8e); 0 = off
 };
 
 struct ParseOutcome {

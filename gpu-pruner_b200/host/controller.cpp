@@ -99,14 +99,16 @@ class FileSource : public WindowSource {
     const int64_t S = ingestor_ ? args.query_slice : 0;
     // daemon mode with a resident window: ask only for what was scraped since the previous tick
     const int64_t since = can_reside ? ingestor_->resident_t_end() : 0;
+    // --late-seconds: the delta also asks again for the newest L seconds the resident window holds
+    const int64_t L = can_reside ? args.late_seconds : 0;
     const bool delta_there = file_exists(base + "/delta/util.json") || (S > 0 && file_exists(base + "/delta/slice-0000"));
     if (since > 0 && delta_there && file_exists(base + "/delta/query.json")) {
       const Json meta = Json::parse_file(base + "/delta/query.json");
       const int64_t start = (int64_t)meta["start"].as_number(0), end = (int64_t)meta["end"].as_number(0);
-      if (start == since && end > start) {
+      if (start == since - L && end > since) {
         try {
-          if (S > 0 && end - start > S) return load_slices(args, base + "/delta", start, end, S, true);
-          return load(args, base + "/delta", end - start, true);
+          if (S > 0 && end - start > S) return load_slices(args, base + "/delta", start, end, S, true, L);
+          return load(args, base + "/delta", end - since, true, L);
         } catch (const NeedFullWindow& e) {
           if (log_) log_->info(std::string("Resident window rebuilt from the full range: ") + e.what());
         }
@@ -125,7 +127,17 @@ class FileSource : public WindowSource {
   }
 
  private:
-  Window load(const Cli& args, const std::string& d, int64_t slice_seconds, bool resident) {
+  // --late-seconds: what the re-ask of a delta tick changed, one line and a counter per tick that raised a cell
+  void log_late(const Window& w, int64_t reask) const {
+    const uint64_t u = w.stats.late_util_cells, p = w.stats.late_power_cells;
+    if (!log_ || u + p == 0) return;
+    char line[200];
+    snprintf(line, sizeof line, "Late samples raised %llu util cells and %llu power cells in the re-asked %lld s",
+             (unsigned long long)u, (unsigned long long)p, (long long)reask);
+    log_->counter("INFO", "monotonic_counter.late_cells", u + p, line);
+  }
+
+  Window load(const Cli& args, const std::string& d, int64_t slice_seconds, bool resident, int64_t reask = 0) {
     const std::string up = d + "/util.json";
     if (!file_exists(up)) throw std::runtime_error("Failed to run query! " + up + " not found");
     const auto read_t0 = std::chrono::steady_clock::now();
@@ -146,6 +158,7 @@ class FileSource : public WindowSource {
       opt.step = (int64_t)meta["step"].as_number(0);
     }
     opt.slice_seconds = slice_seconds;
+    opt.reask_seconds = reask;
     opt.resident = resident;
     opt.reshape = args.reshape_ring;
     if (log_) {
@@ -163,6 +176,7 @@ class FileSource : public WindowSource {
       if (log_ && !w.stats.ring_reshape.empty())  // --reshape-ring: one line per reshape, with its counter
         log_->counter("INFO", "monotonic_counter.ring_reshapes", 1, w.stats.ring_reshape);
       if (log_ && !note.empty()) log_->info(note);
+      log_late(w, reask);
     }
     // node_type for the rows of PodMetricData: the node_dmi_info join of query.promql.j2:23-34
     if (file_exists(d + "/dmi.json")) apply_node_types(w, Json::parse_file(d + "/dmi.json"));
@@ -173,7 +187,8 @@ class FileSource : public WindowSource {
   // ... each with util.json [prof.json] [power.json] and query.json = {"start", "end", "step"} of that query.  A slice
   // that is missing or answers another range fails the query; the session is cold then (ingest_slices reads the
   // slices one by one, after it has given up the resident window).
-  Window load_slices(const Cli& args, const std::string& d, int64_t start, int64_t end, int64_t S, bool delta) {
+  Window load_slices(const Cli& args, const std::string& d, int64_t start, int64_t end, int64_t S, bool delta,
+                     int64_t reask = 0) {
     if (!file_exists(d + "/query.json")) throw std::runtime_error("Failed to run query! " + d + "/query.json not found");
     const int64_t step = (int64_t)Json::parse_file(d + "/query.json")["step"].as_number(0);
     if (step <= 0 || S % step != 0)
@@ -213,7 +228,8 @@ class FileSource : public WindowSource {
     opt.duration_min = args.duration;
     opt.power_threshold = want_power ? *args.power_threshold : 0.0;
     opt.t_end = end, opt.step = step;
-    opt.slice_seconds = delta ? end - start : 0;
+    opt.slice_seconds = delta ? end - start - reask : 0;
+    opt.reask_seconds = delta ? reask : 0;
     opt.resident = true;
     opt.reshape = args.reshape_ring;
     std::string note;
@@ -225,6 +241,7 @@ class FileSource : public WindowSource {
       log_->info(rbuf);
       if (!note.empty()) log_->info(note);
     }
+    log_late(w, opt.reask_seconds);
     if (file_exists(d + "/dmi.json")) apply_node_types(w, Json::parse_file(d + "/dmi.json"));
     return w;
   }

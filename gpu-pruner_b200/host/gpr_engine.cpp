@@ -168,6 +168,7 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
       else
         snprintf(buf, sizeof buf, "Device ingest not used (%s): CPU text parser, %.1f ms", rep.reason.c_str(), ms);
       *note = buf;
+      if (rep.on_device && opt.slice_seconds > 0 && opt.reask_seconds > 0) *note += reask_note(opt, w);
     }
     return w;
   }
@@ -191,8 +192,17 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
                (unsigned long long)rep.ring_growths, (unsigned long long)rep.hard_spans,
                (unsigned long long)rep.rows_patched, rep.scan_ms, rep.labels_ms, rep.assign_ms, rep.parse_ms);
       *note = buf;
+      if (opt.slice_seconds > 0 && opt.reask_seconds > 0) *note += reask_note(opt, w);
     }
     return w;
+  }
+
+  // --late-seconds: what the re-ask cost on top of the tick's own slice
+  static std::string reask_note(const IngestOptions& opt, const Window& w) {
+    char buf[160];
+    snprintf(buf, sizeof buf, "; re-asked the newest %lld s, band read and compare %.2f ms", (long long)opt.reask_seconds,
+             w.stats.band_ms);
+    return buf;
   }
 
  private:
@@ -260,6 +270,11 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
   void resident_live_rows(std::vector<uint32_t>* bits) override {
     bits->assign(((size_t)resident_rows_ + 31) / 32, 0u);
     check(gpr_resident_live_rows(ctx_, bits->data(), GPR_MEM_HOST), "gpr_resident_live_rows");
+  }
+  // --late-seconds: the re-asked band comes back to the host, before and after the tick's merge
+  void resident_cols(int plane, uint32_t newer, uint32_t n_cols, std::vector<float>* out) override {
+    out->resize((size_t)resident_rows_ * n_cols);
+    check(gpr_resident_cols(ctx_, plane, newer, n_cols, out->data(), GPR_MEM_HOST), "gpr_resident_cols");
   }
   // Snapshots: the encoder writes into device buffers kept across ticks, then one copy per array lands in pinned host
   // memory (the two are timed apart).  Capacities carry a quarter of head-room, so a steady tick encodes once; a

@@ -400,11 +400,68 @@ std::string reshape_ring(TextDevice& dev, Window& w, Assigner& asg, uint32_t* po
   return line;
 }
 
+// IngestOptions::reask_seconds: the ring's re-asked buckets as they were before the tick's merge — the n_re buckets that
+// end n_new (the buckets this tick opens) before the newest — per resident plane, read once the ring's shape for the
+// tick is known.  A row is found by (pod, slot): a ring that grows on the way keeps every pod's number, and a row it
+// did not have when the band was read holds no sample.
+struct ReaskBand {
+  uint32_t n_new = 0, n_re = 0, G = 0, rows = 0;
+  std::vector<float> before[2];
+
+  // cell of ring row r (of a ring with G_now slots per pod) `back` buckets before the newest, before the merge
+  float cell(int plane, uint32_t r, uint32_t G_now, uint32_t back) const {
+    const uint32_t pod = r / G_now, slot = r % G_now;
+    const size_t row = (size_t)pod * G + slot;
+    if (slot >= G || row >= rows) return std::numeric_limits<float>::quiet_NaN();
+    return before[plane][row * n_re + (n_new + n_re - 1 - back)];
+  }
+  bool covers(uint32_t back) const { return back >= n_new && back < n_new + n_re; }
+};
+
+void read_band(TextDevice& dev, ReaskBand* band, uint32_t G, int n_planes, IngestStats& st) {
+  const auto t0 = std::chrono::steady_clock::now();
+  band->G = G;
+  for (int k = 0; k < n_planes; ++k) dev.resident_cols(k, band->n_new, band->n_re, &band->before[k]);
+  band->rows = (uint32_t)(band->before[0].size() / band->n_re);
+  st.band_ms += ms_since(t0);
+}
+
+// After the tick's last merge: the cells of the re-asked buckets whose bits changed, per plane — what late samples
+// raised.  (A max never lowers a cell, so every change is a raise.)  Only the rows of the window's pods are compared:
+// the ring's head-room rows have no series.  A row the band did not have when it was read (the ring grew) had no
+// sample there.
+void count_late(TextDevice& dev, const ReaskBand& band, uint32_t n_pods, uint32_t G_now, int n_planes, IngestStats& st) {
+  const auto t0 = std::chrono::steady_clock::now();
+  std::vector<float> after;
+  const uint32_t n_re = band.n_re;
+  for (int k = 0; k < n_planes; ++k) {
+    dev.resident_cols(k, band.n_new, n_re, &after);
+    uint64_t n = 0;
+    const size_t rows = std::min<size_t>(after.size() / n_re, (size_t)n_pods * G_now);
+    for (size_t r = 0; r < rows; ++r) {
+      const uint32_t pod = (uint32_t)(r / G_now), slot = (uint32_t)(r % G_now);
+      const size_t old = (size_t)pod * band.G + slot;
+      const bool had = slot < band.G && old < band.rows;
+      const float* now = after.data() + r * n_re;
+      const float* was = had ? band.before[k].data() + old * n_re : nullptr;
+      for (uint32_t j = 0; j < n_re; ++j) {
+        const bool now_nan = std::isnan(now[j]), was_nan = !was || std::isnan(was[j]);
+        n += !(now_nan && was_nan) && (now_nan != was_nan || memcmp(&was[j], &now[j], sizeof(float)) != 0);
+      }
+    }
+    (k == 0 ? st.late_util_cells : st.late_power_cells) += n;
+  }
+  st.band_ms += ms_since(t0);
+}
+
 // Parses the series of `texts` into plane `plane` (0 util, 1 power) on `grid` (its fill applies to the first text only),
 // then re-parses on the CPU every series feeding a row the device gave up on and writes back that row's buckets of
-// `patch`: a run of patch.T buckets ending at patch.t_end, `newer` buckets before the grid's newest one.
+// `patch`: a run of patch.T buckets ending at patch.t_end, `newer` buckets before the grid's newest one.  Buckets that
+// `band` covers were asked again (IngestOptions::reask_seconds): there the re-parse is merged with what the ring held
+// before the tick (NaN-aware max) instead of overwriting it, so re-asking never lowers a cell.
 void parse_plane(TextDevice& dev, Window& w, const std::vector<TextPlan*>& texts, int plane, TextDevice::TextGrid grid,
-                 const Window& patch, uint32_t newer, double power_threshold, DeviceIngestReport& rep) {
+                 const Window& patch, uint32_t newer, double power_threshold, DeviceIngestReport& rep,
+                 const ReaskBand* band = nullptr) {
   const uint32_t n_rows = grid.n_rows;
   grid.power_threshold = plane == 1 ? power_threshold : 0.0;
   std::vector<uint32_t> writers(n_rows, 0);
@@ -435,6 +492,11 @@ void parse_plane(TextDevice& dev, Window& w, const std::vector<TextPlan*>& texts
   std::vector<uint32_t> row_ids;
   std::vector<int64_t> row_slot(any_dirty ? n_rows : 0, -1);
   const gpr::text::PowerSnap snap = gpr::text::power_snap(plane == 1 ? power_threshold : 0.0);
+  // a bucket without a sample is written back as the fill, the one NaN the device merge raises: a re-asked bucket
+  // (IngestOptions::reask_seconds) may be merged into again by a later tick, and any other NaN would hold off its
+  // samples for good (atomic_merge is an integer max for non-negative values)
+  float no_sample;
+  memcpy(&no_sample, &gpr::text::kFillBits, sizeof no_sample);
   for (size_t k = 0; k < texts.size(); ++k) {
     const std::string& t = *texts[k]->text;
     for (const gpr_text_span& sp : spans[k]) {
@@ -446,7 +508,7 @@ void parse_plane(TextDevice& dev, Window& w, const std::vector<TextPlan*>& texts
       }
       if (row_slot[sp.row] < 0) {
         row_slot[sp.row] = (int64_t)rows.size();
-        rows.emplace_back(patch.T, std::numeric_limits<float>::quiet_NaN());
+        rows.emplace_back(patch.T, no_sample);
         row_ids.push_back(sp.row);
       }
       float* row = rows[(size_t)row_slot[sp.row]].data();
@@ -461,6 +523,12 @@ void parse_plane(TextDevice& dev, Window& w, const std::vector<TextPlan*>& texts
       });
     }
   }
+  if (band)
+    for (size_t i = 0; i < rows.size(); ++i)
+      for (uint32_t c = 0; c < patch.T; ++c) {
+        const uint32_t back = newer + patch.T - 1 - c;
+        if (band->covers(back)) merge_cell(rows[i][c], band->cell(plane, row_ids[i], w.G, back));
+      }
   for (size_t i = 0; i < rows.size(); ++i)
     dev.patch_cols(plane, row_ids[i], w.T, rows[i].data(), patch.T, newer, grid.resident);
   rep.rows_patched += rows.size();
@@ -475,6 +543,8 @@ const char* delta_blocker(const State& st, const IngestOptions& opt, bool with_p
   if (opt.t_end - opt.slice_seconds != st.w.t_end) return "the slice does not start where the resident window ends";
   if (opt.slice_seconds % opt.step != 0) return "the slice is not a whole number of steps";
   if (opt.slice_seconds / opt.step >= (int64_t)st.w.T) return "the slice is as long as the window";
+  if (opt.reask_seconds > 0 && (opt.slice_seconds + opt.reask_seconds + opt.step - 1) / opt.step >= (int64_t)st.w.T)
+    return "the slice and the re-asked seconds are as long as the window";
   if (with_power != st.with_power) return "power plane appeared / disappeared";
   if (with_power && !(opt.power_threshold == st.power_threshold ||
                       (std::isnan(opt.power_threshold) && std::isnan(st.power_threshold))))
@@ -568,6 +638,7 @@ Window DeviceIngestSession::ingest(const std::string& util, const std::string* p
   std::sort(prof_rows.begin(), prof_rows.end());
 
   uint32_t n_new = 0;  // buckets this call opens (delta) — 0: the whole window
+  ReaskBand band;      // IngestOptions::reask_seconds: the re-asked buckets before the merge (n_re == 0: none)
   if (!delta) {
     finish_shape(w, opt, 0, 1, power != nullptr, /*allocate=*/false);  // t_end / step given: nothing to infer
     st.with_power = power != nullptr;
@@ -604,6 +675,15 @@ Window DeviceIngestSession::ingest(const std::string& util, const std::string* p
       }
     }
     w.P = (uint32_t)w.pods.size();
+    if (opt.reask_seconds > 0 && w.P > 0) {
+      band.n_new = n_new, band.n_re = (uint32_t)((opt.reask_seconds + opt.step - 1) / opt.step);
+      try {
+        read_band(dev_, &band, w.G, st.with_power ? 2 : 1, w.stats);
+      } catch (const std::exception& e) {
+        st.valid = false;
+        throw NeedFullWindow(std::string("the re-asked buckets could not be read: ") + e.what());
+      }
+    }
   }
   const bool resident = delta || opt.resident;
   const uint32_t n_rows = (resident ? st.pods_cap : w.P) * w.G;
@@ -620,15 +700,17 @@ Window DeviceIngestSession::ingest(const std::string& util, const std::string* p
 
   // window the parse accepts: the whole range, or only the tick's slice; the CPU re-parse patches the same buckets
   TextDevice::TextGrid grid;
-  grid.t_end = w.t_end, grid.span = delta ? opt.slice_seconds : w.span, grid.step = w.step, grid.T = w.T;
-  grid.n_rows = n_rows, grid.fill = !resident, grid.resident = resident;
+  grid.t_end = w.t_end, grid.span = delta ? opt.slice_seconds + opt.reask_seconds : w.span, grid.step = w.step;
+  grid.T = w.T, grid.n_rows = n_rows, grid.fill = !resident, grid.resident = resident;
   Window patch;
-  patch.t_end = w.t_end, patch.step = w.step, patch.span = grid.span, patch.T = delta ? n_new : w.T;
+  patch.t_end = w.t_end, patch.step = w.step, patch.span = grid.span, patch.T = delta ? n_new + band.n_re : w.T;
+  const ReaskBand* re = band.n_re ? &band : nullptr;
   std::vector<TextPlan*> util_texts;
   if (pl_prof) util_texts.push_back(pl_prof);
   util_texts.push_back(pl_util);
-  parse_plane(dev_, w, util_texts, 0, grid, patch, 0, opt.power_threshold, rep);
-  if (pl_power) parse_plane(dev_, w, {pl_power}, 1, grid, patch, 0, opt.power_threshold, rep);
+  parse_plane(dev_, w, util_texts, 0, grid, patch, 0, opt.power_threshold, rep, re);
+  if (pl_power) parse_plane(dev_, w, {pl_power}, 1, grid, patch, 0, opt.power_threshold, rep, re);
+  if (re) count_late(dev_, band, (uint32_t)w.pods.size(), w.G, st.with_power ? 2 : 1, w.stats);
   rep.on_device = true;
   Window out = result();
   if (!resident) {
@@ -657,7 +739,7 @@ Window DeviceIngestSession::ingest_slices(const SlicedFetch& f, const IngestOpti
   }
   st.valid = false;
   if (opt.t_end <= 0 || opt.step <= 0) throw std::runtime_error("a sliced query needs the window end and step (query.json)");
-  const int64_t span = delta ? opt.slice_seconds : std::max<int64_t>(1, opt.duration_min * 60);
+  const int64_t span = delta ? opt.slice_seconds + opt.reask_seconds : std::max<int64_t>(1, opt.duration_min * 60);
   // the slices must tile (t_end - span, t_end] and meet on the bucket grid
   if (f.ranges.empty() || f.ranges.front().first != opt.t_end - span || f.ranges.back().second != opt.t_end)
     throw std::runtime_error("the query slices do not cover the queried range");
@@ -677,10 +759,21 @@ Window DeviceIngestSession::ingest_slices(const SlicedFetch& f, const IngestOpti
   Window& w = st.w;
   w.stats = IngestStats();
   Assigner& asg = *st.asg;
+  ReaskBand band;  // IngestOptions::reask_seconds: the re-asked buckets before the merge (n_re == 0: none)
   if (delta) {
     w.t_end = opt.t_end;
     dev_.resident_advance((uint32_t)(opt.slice_seconds / opt.step));
+    if (opt.reask_seconds > 0) {
+      band.n_new = (uint32_t)(opt.slice_seconds / opt.step);
+      band.n_re = (uint32_t)((opt.reask_seconds + opt.step - 1) / opt.step);
+      try {
+        read_band(dev_, &band, w.G, st.with_power ? 2 : 1, w.stats);
+      } catch (const std::exception& e) {
+        throw NeedFullWindow(std::string("the re-asked buckets could not be read: ") + e.what());
+      }
+    }
   }
+  const ReaskBand* re = band.n_re ? &band : nullptr;
   // the ring keeps every row it has; new pods and slots get rows of their own
   auto grow = [&](uint32_t pods, uint32_t G) {
     std::vector<uint32_t> src((size_t)pods * G, GPR_ROW_NONE);
@@ -741,9 +834,10 @@ Window DeviceIngestSession::ingest_slices(const SlicedFetch& f, const IngestOpti
       const uint32_t newer = (uint32_t)((w.t_end - patch.t_end) / w.step);
       patch.T = (uint32_t)std::min<int64_t>(w.T - newer, (patch.span + w.step - 1) / w.step);
       grid.n_rows = st.pods_cap * w.G;
-      parse_plane(dev_, w, {&plan}, kind == 2 ? 1 : 0, grid, patch, newer, opt.power_threshold, rep);
+      parse_plane(dev_, w, {&plan}, kind == 2 ? 1 : 0, grid, patch, newer, opt.power_threshold, rep, re);
     }
   }
+  if (re) count_late(dev_, band, (uint32_t)w.pods.size(), w.G, st.with_power ? 2 : 1, w.stats);
   if (!delta) {
     st.prof_rows = prof_rows;
     // the shape a one-query ingest of the range gives the ring, so that later ticks take the same path

@@ -86,6 +86,13 @@ class TextDevice {
     (void)bits;
     throw std::logic_error("this device cannot reshape its ring");
   }
+  // IngestOptions::reask_seconds: plane `plane` of the ring's n_cols buckets that end `newer` buckets before the newest,
+  // oldest first, for every row (gpr_resident_cols: (*out)[r * n_cols + j]).  A device that cannot read a band throws;
+  // the session then takes the full range.
+  virtual void resident_cols(int plane, uint32_t newer, uint32_t n_cols, std::vector<float>* out) {
+    (void)plane, (void)newer, (void)n_cols, (void)out;
+    throw std::logic_error("this device cannot read a band of its ring");
+  }
 };
 
 struct DeviceIngestReport {

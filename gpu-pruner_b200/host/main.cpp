@@ -46,6 +46,10 @@ int main(int argc, char** argv) {
     log.warn("--query-slice ignored: slicing needs the device ingest (GPR_INGEST=cpu asks for whole ranges)");
     run.query_slice = 0;
   }
+  if (cpu_ingestor && run.late_seconds > 0) {
+    log.warn("--late-seconds ignored: GPR_INGEST=cpu keeps no resident window and asks for the full range every tick");
+    run.late_seconds = 0;
+  }
   std::unique_ptr<gph::WindowSource> src = gph::make_window_source(cli.prometheus_url, ingestor, &log);
   gph::Controller ctl(run, kube.get(), engine.get(), log, gph::system_clock());
   // --snapshot-file: the resident window survives a restart (snapshot.hpp).  The CPU ingest keeps no resident window,

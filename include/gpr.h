@@ -307,6 +307,17 @@ GPR_API int gpr_resident_remap(gpr_ctx *ctx, uint32_t n_pods, uint32_t n_gpus, c
  * slice, and gpr_resident_remap the kept pods' rows (and GPR_ROW_NONE for the new ones) into
  * [kept + head-room][max(G, slots needed)]; then append the slice as on any tick.                    */
 GPR_API int gpr_resident_live_rows(gpr_ctx *ctx, uint32_t *bits, int32_t mem_kind);
+/* out[r * n_cols + j] = plane `plane` of ring row r at the bucket (n_cols - 1 - j + newer) back from the newest:
+ * the n_cols buckets that end `newer` buckets before the newest, oldest first, for every ring row (n_pods * n_gpus).
+ * Cells are copied as bits (a NaN is "no sample").  Host or device output (mem_kind); a host one goes through
+ * context scratch and is copied out once.  Blocking, reads the ring only; decisions enqueued before it stay
+ * pending.  No resident window, or plane 1 on a ring without a power plane, is GPR_E_STATE; a plane other than
+ * 0 or 1, n_cols == 0, newer + n_cols > n_samples, a NULL out or a bad mem_kind GPR_E_INVALID; on any error out
+ * is untouched.
+ * A daemon caller that re-asks the newest L seconds it already holds (samples that reached the server late)
+ * reads the re-asked band before and after the tick's merge to see what the late samples changed.           */
+GPR_API int gpr_resident_cols(gpr_ctx *ctx, int32_t plane, uint32_t newer, uint32_t n_cols, float *out,
+                              int32_t mem_kind);
 
 /* ---- multi-GPU: one process per GPU, pods sharded by rank, one allgather of the bitmap - */
 #define GPR_UNIQUE_ID_BYTES 128
