@@ -1553,6 +1553,56 @@ int gpr_resident_cols(gpr_ctx* ctx, int32_t plane, uint32_t newer, uint32_t n_co
   GPR_CATCH(ctx)
 }
 
+int gpr_resident_retime(gpr_ctx* ctx, uint32_t n_keep, uint32_t factor) {
+  if (!ctx) return GPR_E_INVALID;
+  GPR_TRY
+  NvtxRange nvtx_range("gpr_resident_retime");
+  if (const int rc = enter(ctx)) return rc;
+  if (!ctx->d_res_util) return fail(ctx, GPR_E_STATE, "no resident window (gpr_resident_init)");
+  if (factor == 0) return fail(ctx, GPR_E_INVALID, "factor is 0");
+  if (n_keep == 0 || n_keep > ctx->res_T)
+    return fail(ctx, GPR_E_INVALID, "n_keep = %u: the resident window has %u samples", n_keep, ctx->res_T);
+  // ---- the new ring beside the old one, gathered on the stream after whatever is enqueued there (the decisions still
+  // pending read the old ring); they change places only once it is complete
+  const uint32_t T_new = gpr::retime_len(n_keep, factor);
+  const uint32_t rows = ctx->res_P * ctx->res_G;
+  const bool index = ctx->d_idx_util != nullptr;
+  const uint32_t ld_new = index ? gpr::index_ld(T_new) : 0;
+  Buf<float>* cur[2] = {&ctx->d_res_util, &ctx->d_res_power};
+  int rc = GPR_OK;
+  for (int k = 0; k < 2 && rc == GPR_OK; ++k) {
+    if (!*cur[k]) continue;
+    Buf<float>& plane = ctx->d_res_next[k];
+    Buf<float>& idx = ctx->d_res_next[2 + k];
+    cudaError_t e = plane.alloc((size_t)rows * T_new);
+    if (e == cudaSuccess && index) e = idx.alloc((size_t)rows * ld_new);
+    if (e != cudaSuccess) {
+      rc = fail(ctx, e == cudaErrorMemoryAllocation ? GPR_E_NOMEM : GPR_E_CUDA, "gpr_resident_retime: %s",
+                cudaGetErrorString(e));
+      break;
+    }
+    rc = launch(ctx, gpr::k_retime_rows, gpr::ring_grid(rows, ctx->sm_count), gpr::kRingThreads, 0, false,
+                reinterpret_cast<uint32_t*>(plane.p), reinterpret_cast<const uint32_t*>(cur[k]->p), rows, ctx->res_T,
+                ctx->res_head, n_keep, factor, index ? idx.p : nullptr, ld_new);
+  }
+  if (rc == GPR_OK) {
+    const cudaError_t e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) rc = fail(ctx, GPR_E_CUDA, "gpr_resident_retime: %s", cudaGetErrorString(e));
+  }
+  if (rc != GPR_OK) {
+    (void)cudaStreamSynchronize(ctx->stream);  // a gather may still be writing a new buffer
+    for (Buf<float>& b : ctx->d_res_next) (void)b.release();
+    return rc;
+  }
+  Buf<float>* all[4] = {&ctx->d_res_util, &ctx->d_res_power, &ctx->d_idx_util, &ctx->d_idx_power};
+  for (int k = 0; k < 4; ++k) all[k]->swap(ctx->d_res_next[k]);
+  ctx->res_T = T_new, ctx->res_head = 0;
+  if (index) ctx->idx_ld = ld_new, ctx->idx_stale = false;  // rebuilt from the new planes
+  for (Buf<float>& b : ctx->d_res_next) CU(b.release());    // the old ring
+  return GPR_OK;
+  GPR_CATCH(ctx)
+}
+
 int gpr_resident_planes(gpr_ctx* ctx, float** util, float** power, uint64_t* row_stride) {
   if (!ctx) return GPR_E_INVALID;
   if (!ctx->d_res_util) return fail(ctx, GPR_E_STATE, "no resident window");

@@ -6,7 +6,8 @@
 // row length) is plain functions.  gpr_api.cu launches what these return; tests/cpp/ring_emul.cpp runs the same
 // source on the CPU against a numpy model of the ring.  gpr_resident_remap's row gather and map check are here too
 // (tests/cpp/remap_emul.cpp), gpr_resident_live_rows' row test (tests/cpp/live_rows_emul.cpp) and gpr_resident_cols'
-// band gather (tests/cpp/ring_cols_emul.cpp).
+// band gather (tests/cpp/ring_cols_emul.cpp), and gpr_resident_retime's regrouping of the newest buckets
+// (tests/cpp/retime_emul.cpp).
 #pragma once
 
 #include <stddef.h>
@@ -307,6 +308,75 @@ __global__ void __launch_bounds__(kRingThreads) k_ring_cols(uint32_t* __restrict
       uint32_t t = start + j;
       if (t >= T) t -= T;
       o[j] = in[t];
+    }
+  }
+}
+
+// ---- gpr_resident_retime: the ring's newest n_keep buckets regrouped `factor` to a bucket, out of place.  Whether a
+// change of step and window is exact, and what n_keep and factor it takes, is gpr::retime_plan (gpr_retime.h).
+// Row length after the retime: ceil(n_keep / factor).
+inline uint32_t retime_len(uint32_t n_keep, uint32_t factor) { return (n_keep + factor - 1) / factor; }
+
+// A cell's bits as an int whose order is the float order, with -0 below +0: keys of non-negative floats are their bits,
+// keys of negative ones have the magnitude bits flipped.  The map is its own inverse.  Comparing keys instead of floats
+// keeps denormals exact whatever the float compare flushes.
+__device__ __forceinline__ int32_t retime_key(uint32_t b) {
+  return (int32_t)(b ^ ((uint32_t)((int32_t)b >> 31) >> 1));
+}
+
+// New cell of one group: the maximum of the n old cells at ring positions t, t + 1, ... (mod T), as text::atomic_merge
+// leaves a fill cell that took them in any order — every NaN is no sample, a group without one is kNoSampleBits, and
+// +0 beats -0.  Every finite or infinite key is above INT32_MIN.
+__device__ __forceinline__ uint32_t retime_group(const uint32_t* __restrict__ row, uint32_t T, uint32_t t, uint32_t n) {
+  int32_t best = INT32_MIN;
+  for (uint32_t j = 0; j < n; ++j) {
+    const uint32_t b = row[t];
+    if (has_sample_bits(b)) best = max(best, retime_key(b));
+    if (++t == T) t = 0;
+  }
+  return best == INT32_MIN ? kNoSampleBits : (uint32_t)retime_key((uint32_t)best);
+}
+
+// New position p (0 = oldest) of a retimed row: new bucket T' - 1 - p is old buckets [k b', min(k b' + k, n_keep))
+// counted from the newest, which sits at ring position head + T - 1; the group is read oldest first.
+__device__ __forceinline__ uint32_t retime_cell(const uint32_t* __restrict__ row, uint32_t T, uint32_t head,
+                                                uint32_t n_keep, uint32_t factor, uint32_t T_new, uint32_t p) {
+  const uint32_t lo = (T_new - 1 - p) * factor, hi = min(lo + factor, n_keep);  // old buckets [lo, hi)
+  return retime_group(row, T, (uint32_t)(((uint64_t)head + T - hi) % T), hi - lo);
+}
+
+// One new row per CTA and round (grid: ring_grid): old row r of length T with its head at `head` becomes new row r of
+// length T_new = retime_len(n_keep, factor), oldest first (its head is 0).  Lane i of a warp takes new cell i, so a warp's
+// loads of one group step cover 32 groups `factor` words apart and the later steps find those lines in L1.  16-byte stores
+// when new rows start on a 16-byte boundary (T_new % 4 == 0), 4-byte ones otherwise.  With an index (idx, of rows
+// idx_ld long), the CTA then rebuilds the row's blocks from the row it wrote and sets the padding to no sample.
+__global__ void __launch_bounds__(kRingThreads) k_retime_rows(uint32_t* __restrict__ dst, const uint32_t* __restrict__ src,
+                                                              uint32_t n_rows, uint32_t T, uint32_t head, uint32_t n_keep,
+                                                              uint32_t factor, float* __restrict__ idx, uint32_t idx_ld) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+  const uint32_t T_new = (n_keep + factor - 1) / factor;  // retime_len
+  for (uint32_t r = blockIdx.x; r < n_rows; r += gridDim.x) {
+    const uint32_t* in = src + (size_t)r * T;
+    uint32_t* out = dst + (size_t)r * T_new;
+    if (T_new % 4u == 0) {
+      uint4* out4 = reinterpret_cast<uint4*>(out);
+      for (uint32_t j = threadIdx.x; j < T_new / 4u; j += blockDim.x) {
+        const uint32_t p = 4u * j;
+        out4[j] = make_uint4(retime_cell(in, T, head, n_keep, factor, T_new, p),
+                             retime_cell(in, T, head, n_keep, factor, T_new, p + 1),
+                             retime_cell(in, T, head, n_keep, factor, T_new, p + 2),
+                             retime_cell(in, T, head, n_keep, factor, T_new, p + 3));
+      }
+    } else {
+      for (uint32_t p = threadIdx.x; p < T_new; p += blockDim.x) out[p] = retime_cell(in, T, head, n_keep, factor, T_new, p);
+    }
+    if (idx) {
+      float* idx_row = idx + (size_t)r * idx_ld;
+      __syncthreads();  // this CTA's stores to the row are visible to its own warps
+      recompute_blocks(reinterpret_cast<const float*>(out), T_new, 0, T_new, idx_row, warp, n_warps, lane);
+      for (uint32_t b = (T_new + kIdxBlock - 1) / kIdxBlock + threadIdx.x; b < idx_ld; b += blockDim.x)
+        reinterpret_cast<uint32_t*>(idx_row)[b] = kNoSampleBits;
+      __syncthreads();
     }
   }
 }

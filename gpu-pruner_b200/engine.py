@@ -577,6 +577,12 @@ class IdleEngine:
         self._check(self._lib.gpr_resident_live_rows(self._h, words.ctypes.data, ffi.GPR_MEM_HOST))
         return np.unpackbits(words.view(np.uint8), bitorder="little")[:rows].astype(bool)
 
+    def resident_retime(self, n_keep: int, factor: int):
+        """Put the resident ring on a coarser or shorter grid (gpr_resident_retime): its newest ``n_keep`` buckets
+        merged ``factor`` to a bucket, newest first, into ``ceil(n_keep / factor)`` buckets; the head becomes 0 and a
+        block index is rebuilt.  ``gpr::retime_plan`` (csrc/gpr_retime.h) says which grid changes this makes exact."""
+        self._check(self._lib.gpr_resident_retime(self._h, int(n_keep), int(factor)))
+
     def resident_cols(self, plane: int, newer: int, n_cols: int) -> np.ndarray:
         """A band of the resident ring (gpr_resident_cols): the ``n_cols`` buckets that end ``newer`` buckets before
         the newest, oldest first, of plane ``plane`` (0 util, 1 power) for every row — a float32 array

@@ -135,6 +135,7 @@ PROTOTYPES = {
     "gpr_resident_remap": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P, C.c_int32]),
     "gpr_resident_live_rows": (C.c_int, [_P, _P, C.c_int32]),
     "gpr_resident_cols": (C.c_int, [_P, C.c_int32, C.c_uint32, C.c_uint32, _P, C.c_int32]),
+    "gpr_resident_retime": (C.c_int, [_P, C.c_uint32, C.c_uint32]),
     "gpr_comm_unique_id": (C.c_int, [_P]),
     "gpr_comm_init": (C.c_int, [_P, _P, C.c_int, C.c_int]),
     "gpr_comm_destroy": (C.c_int, [_P]),

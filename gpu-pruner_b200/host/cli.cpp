@@ -45,6 +45,7 @@ std::string usage() {
       "      --gpu-device <N>                       (extension) CUDA device ordinal [default: 0]\n"
       "      --snapshot-file <PATH>                 (extension) with -d: save the resident window after every tick, resume from it at start\n"
       "      --reshape-ring                         (extension) with -d: reshape the resident window on the GPU when pods or GPU slots outgrow it\n"
+      "      --retime-ring                          (extension) with -d: retime the resident window on the GPU when the query step grows by a whole factor or --duration shrinks\n"
       "      --query-slice <SECONDS>                (extension) ask ranges longer than this as consecutive queries of at most this length, merged on the GPU; no CPU-parser fallback for slices [default: 0 = one query]\n"
       "      --late-seconds <SECONDS>               (extension) with -d: ask every tick again for the newest SECONDS of the resident window, so samples that reach Prometheus late still count [default: 0 = off]\n"
       "  -h, --help                                 Print help\n";
@@ -143,6 +144,7 @@ ParseOutcome parse_cli(const std::vector<std::string>& args) {
   }};
   specs["snapshot-file"] = {0, true, [&](const std::string& v) { c.snapshot_file = v; return std::string(); }};
   specs["reshape-ring"] = {0, false, [&](const std::string&) { c.reshape_ring = true; return std::string(); }};
+  specs["retime-ring"] = {0, false, [&](const std::string&) { c.retime_ring = true; return std::string(); }};
   specs["query-slice"] = {0, true, [&](const std::string& v) {
     uint64_t x = 0;
     std::string e = parse_u64(v, &x);
@@ -224,6 +226,8 @@ ParseOutcome parse_cli(const std::vector<std::string>& args) {
     return fail("the argument '--snapshot-file <PATH>' can only be used with '--daemon-mode'");
   if (c.reshape_ring && !c.daemon_mode)
     return fail("the argument '--reshape-ring' can only be used with '--daemon-mode'");
+  if (c.retime_ring && !c.daemon_mode)
+    return fail("the argument '--retime-ring' can only be used with '--daemon-mode'");
   if (late_given && !c.daemon_mode)
     return fail("the argument '--late-seconds <SECONDS>' can only be used with '--daemon-mode'");
   if (c.late_seconds > 0 && c.late_seconds >= c.duration * 60)

@@ -42,6 +42,9 @@ struct Cli {
   bool reshape_ring = false;                  // --reshape-ring (-d only): a tick whose cluster outgrew the resident
                                               // window's shape reshapes it on the GPU instead of querying the full
                                               // range (DESIGN.md §8e)
+  bool retime_ring = false;                   // --retime-ring (-d only): a tick whose query step grew by a whole factor,
+                                              // or whose --duration got shorter, retimes the resident window on the GPU
+                                              // instead of querying the full range (DESIGN.md §8e)
   int64_t query_slice = 0;                    // --query-slice SECONDS: a range longer than this is asked as consecutive
                                               // queries of at most this length, merged into the resident window on the
                                               // GPU (DESIGN.md §8e); 0 = one query per range

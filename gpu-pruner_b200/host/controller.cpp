@@ -127,6 +127,11 @@ class FileSource : public WindowSource {
   }
 
  private:
+  // --retime-ring: one line per retime, with its counter
+  void log_retime(const Window& w) const {
+    if (log_ && !w.stats.ring_retime.empty()) log_->counter("INFO", "monotonic_counter.ring_retimes", 1, w.stats.ring_retime);
+  }
+
   // --late-seconds: what the re-ask of a delta tick changed, one line and a counter per tick that raised a cell
   void log_late(const Window& w, int64_t reask) const {
     const uint64_t u = w.stats.late_util_cells, p = w.stats.late_power_cells;
@@ -161,6 +166,7 @@ class FileSource : public WindowSource {
     opt.reask_seconds = reask;
     opt.resident = resident;
     opt.reshape = args.reshape_ring;
+    opt.retime = args.retime_ring;
     if (log_) {
       char rbuf[160];
       snprintf(rbuf, sizeof rbuf, "Recorded responses read from %s: %.1f MB in %.1f ms", d.c_str(), read_bytes / 1e6,
@@ -173,6 +179,7 @@ class FileSource : public WindowSource {
     } else {
       std::string note;
       w = ingestor_->ingest(args, util, pprof, ppower, opt, &note);
+      log_retime(w);
       if (log_ && !w.stats.ring_reshape.empty())  // --reshape-ring: one line per reshape, with its counter
         log_->counter("INFO", "monotonic_counter.ring_reshapes", 1, w.stats.ring_reshape);
       if (log_ && !note.empty()) log_->info(note);
@@ -232,8 +239,10 @@ class FileSource : public WindowSource {
     opt.reask_seconds = delta ? reask : 0;
     opt.resident = true;
     opt.reshape = args.reshape_ring;
+    opt.retime = args.retime_ring;
     std::string note;
     Window w = ingestor_->ingest_slices(args, f, opt, &note);
+    log_retime(w);
     if (log_) {
       char rbuf[200];
       snprintf(rbuf, sizeof rbuf, "Recorded responses read from %s: %zu query slices of at most %lld s, %.1f MB in %.1f ms",

@@ -271,6 +271,10 @@ class GprVerdictEngine : public VerdictEngine, public TextIngestor, private Text
     bits->assign(((size_t)resident_rows_ + 31) / 32, 0u);
     check(gpr_resident_live_rows(ctx_, bits->data(), GPR_MEM_HOST), "gpr_resident_live_rows");
   }
+  // --retime-ring: the rows stay, only their length and the head change
+  void resident_retime(uint32_t n_keep, uint32_t factor) override {
+    check(gpr_resident_retime(ctx_, n_keep, factor), "gpr_resident_retime");
+  }
   // --late-seconds: the re-asked band comes back to the host, before and after the tick's merge
   void resident_cols(int plane, uint32_t newer, uint32_t n_cols, std::vector<float>* out) override {
     out->resize((size_t)resident_rows_ * n_cols);

@@ -71,6 +71,8 @@ struct IngestStats {
   std::vector<std::string> warnings;
   // daemon mode with IngestOptions::reshape: what reshaping the resident ring did this tick ("" = it was not reshaped)
   std::string ring_reshape;
+  // daemon mode with IngestOptions::retime: what retiming the resident ring did this tick ("" = it was not retimed)
+  std::string ring_retime;
   // daemon mode with IngestOptions::reask_seconds: cells of the re-asked buckets whose bits the tick changed, per plane
   // (late samples), and the time spent reading the band before and after the merge
   uint64_t late_util_cells = 0, late_power_cells = 0;
@@ -112,6 +114,10 @@ struct IngestOptions {
   // beyond its G, reshapes the ring on the GPU (gpr_resident_live_rows + gpr_resident_remap) instead of throwing
   // NeedFullWindow; pods without a sample left in the window are dropped then
   bool reshape = false;
+  // daemon mode (--retime-ring): a delta tick whose step grew by a whole factor, or whose window got shorter on an edge
+  // of the old step's buckets, retimes the ring on the GPU (gpr::retime_plan, gpr_resident_retime) instead of throwing
+  // NeedFullWindow; every other change of step or window still throws
+  bool retime = false;
   // daemon mode (--late-seconds): a delta's responses cover (t_end - slice_seconds - reask_seconds, t_end]: the newest
   // reask_seconds the ring already holds are asked again, so samples that reached the server late are merged in (a
   // NaN-aware max, so a sample seen twice leaves its cell as it was).  Only slice_seconds / step buckets are opened.

@@ -16,6 +16,7 @@
 #include <mutex>
 #include <thread>
 
+#include "../csrc/gpr_retime.h"
 #include "ingest_internal.hpp"
 
 namespace gph {
@@ -534,12 +535,14 @@ void parse_plane(TextDevice& dev, Window& w, const std::vector<TextPlan*>& texts
   rep.rows_patched += rows.size();
 }
 
+constexpr const char* kGridChanged = "step / window length changed";
+
 // The first failing check of a delta tick against the resident window (nullptr: the ring can take the tick): same
-// grid, contiguous with what is resident, the same power plane
+// grid (unless `grid` is false: the checks after a retime), contiguous with what is resident, the same power plane
 template <typename State>
-const char* delta_blocker(const State& st, const IngestOptions& opt, bool with_power) {
+const char* delta_blocker(const State& st, const IngestOptions& opt, bool with_power, bool grid = true) {
   if (!st.valid) return "nothing resident";
-  if (opt.step != st.w.step || opt.duration_min * 60 != st.w.span) return "step / window length changed";
+  if (grid && (opt.step != st.w.step || opt.duration_min * 60 != st.w.span)) return kGridChanged;
   if (opt.t_end - opt.slice_seconds != st.w.t_end) return "the slice does not start where the resident window ends";
   if (opt.slice_seconds % opt.step != 0) return "the slice is not a whole number of steps";
   if (opt.slice_seconds / opt.step >= (int64_t)st.w.T) return "the slice is as long as the window";
@@ -550,6 +553,52 @@ const char* delta_blocker(const State& st, const IngestOptions& opt, bool with_p
                       (std::isnan(opt.power_threshold) && std::isnan(st.power_threshold))))
     return "the power threshold changed";
   return nullptr;
+}
+
+// IngestOptions::retime: a delta tick whose only failing check is the grid's.  When gpr::retime_plan finds the change
+// exact (a step that grew by a whole factor, a window that got shorter on an old bucket edge), the session takes the new
+// grid, the other checks are evaluated against it, and the ring is retimed on the GPU (gpr_resident_retime).  Every
+// PROF-fed row must still hold a sample: a fresh query of the new window would stop shadowing the UTIL twin of one
+// that does not, and those UTIL samples were never parsed.  Returns the log line; anything else throws NeedFullWindow
+// with the session invalid, and the tick takes the full range.
+template <typename State>
+std::string retime_ring(TextDevice& dev, State& st, const IngestOptions& opt, bool with_power) {
+  Window& w = st.w;
+  auto refuse = [&st](const std::string& why) {
+    st.valid = false;
+    throw NeedFullWindow(why);
+  };
+  const int64_t N_old = w.span, s_old = w.step, N_new = std::max<int64_t>(1, opt.duration_min * 60);
+  const uint32_t T_old = w.T;
+  const gpr::RetimePlan plan = gpr::retime_plan(N_old, s_old, T_old, N_new, opt.step);
+  if (plan.refusal) refuse(std::string(kGridChanged) + " (" + plan.refusal + ")");
+  w.step = opt.step, w.span = N_new, w.T = (plan.n_keep + plan.factor - 1) / plan.factor;
+  if (const char* why = delta_blocker(st, opt, with_power, /*grid=*/false)) refuse(why);
+  const auto t0 = std::chrono::steady_clock::now();
+  try {
+    dev.resident_retime(plan.n_keep, plan.factor);
+  } catch (const std::exception& e) {  // GPR_E_NOMEM included (the peak is the old ring plus the new one)
+    refuse(std::string("the resident window could not be retimed: ") + e.what());
+  }
+  const double retime_ms = ms_since(t0);
+  if (!st.prof_rows.empty()) {
+    std::vector<uint32_t> bits;
+    try {
+      dev.resident_live_rows(&bits);
+    } catch (const std::exception& e) {
+      refuse(std::string("the live rows of the retimed window could not be read: ") + e.what());
+    }
+    for (const auto& pr : st.prof_rows) {
+      const size_t r = (size_t)pr.first * w.G + pr.second;
+      if (r / 32 >= bits.size() || !((bits[r / 32] >> (r % 32)) & 1u))
+        refuse("a DCGM_FI_PROF_GR_ENGINE_ACTIVE series has no sample left in the retimed window");
+    }
+  }
+  char line[200];
+  snprintf(line, sizeof line,
+           "Resident window retimed on the GPU: %u -> %u (step %lld -> %lld s, window %lld -> %lld s, retime %.2f ms)",
+           T_old, w.T, (long long)s_old, (long long)w.step, (long long)N_old, (long long)w.span, retime_ms);
+  return line;
 }
 
 uint32_t slots_needed(const Window& w) {
@@ -592,11 +641,15 @@ Window DeviceIngestSession::ingest(const std::string& util, const std::string* p
   };
   if (opt.t_end <= 0 || opt.step <= 0) return cpu("window end / step not given (query.json)");
 
+  std::string retimed;  // IngestOptions::retime: the log line of this tick's retime ("" = none)
   if (delta) {
     // what must hold for the ring to take this tick: same grid, contiguous with what is resident
     if (const char* why = delta_blocker(st, opt, power != nullptr)) {
-      st.valid = false;
-      throw NeedFullWindow(why);
+      if (!(opt.retime && why == kGridChanged)) {
+        st.valid = false;
+        throw NeedFullWindow(why);
+      }
+      retimed = retime_ring(dev_, st, opt, power != nullptr);
     }
     // From here on the session's rows and the ring are being changed: whatever interrupts this tick (a device error
     // in the parse, a malformed slice) must not leave a ring that claims to hold the window ending at this tick —
@@ -610,6 +663,7 @@ Window DeviceIngestSession::ingest(const std::string& util, const std::string* p
   }
   Window& w = st.w;
   w.stats = IngestStats();
+  w.stats.ring_retime = retimed;
   Assigner& asg = *st.asg;
 
   TextPlan plans[3];  // prof, util, power — the order the CPU paths assign rows in
@@ -731,10 +785,14 @@ Window DeviceIngestSession::ingest_slices(const SlicedFetch& f, const IngestOpti
   rep = DeviceIngestReport{};
   State& st = *st_;
   const bool delta = opt.slice_seconds > 0;
+  std::string retimed;  // IngestOptions::retime: the log line of this tick's retime ("" = none)
   if (delta) {
     if (const char* why = delta_blocker(st, opt, f.has_power)) {
-      st.valid = false;
-      throw NeedFullWindow(why);
+      if (!(opt.retime && why == kGridChanged)) {
+        st.valid = false;
+        throw NeedFullWindow(why);
+      }
+      retimed = retime_ring(dev_, st, opt, f.has_power);
     }
   }
   st.valid = false;
@@ -758,6 +816,7 @@ Window DeviceIngestSession::ingest_slices(const SlicedFetch& f, const IngestOpti
   }
   Window& w = st.w;
   w.stats = IngestStats();
+  w.stats.ring_retime = retimed;
   Assigner& asg = *st.asg;
   ReaskBand band;  // IngestOptions::reask_seconds: the re-asked buckets before the merge (n_re == 0: none)
   if (delta) {

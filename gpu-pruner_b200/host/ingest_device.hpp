@@ -86,6 +86,13 @@ class TextDevice {
     (void)bits;
     throw std::logic_error("this device cannot reshape its ring");
   }
+  // IngestOptions::retime: the ring's newest n_keep buckets merged `factor` to a bucket (gpr_resident_retime, with the
+  // arguments gpr::retime_plan gives); the rows and the power plane stay, the head becomes 0.  A device that cannot
+  // retime throws; the session then takes the full range.
+  virtual void resident_retime(uint32_t n_keep, uint32_t factor) {
+    (void)n_keep, (void)factor;
+    throw std::logic_error("this device cannot retime its ring");
+  }
   // IngestOptions::reask_seconds: plane `plane` of the ring's n_cols buckets that end `newer` buckets before the newest,
   // oldest first, for every row (gpr_resident_cols: (*out)[r * n_cols + j]).  A device that cannot read a band throws;
   // the session then takes the full range.

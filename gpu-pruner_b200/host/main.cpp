@@ -50,6 +50,10 @@ int main(int argc, char** argv) {
     log.warn("--late-seconds ignored: GPR_INGEST=cpu keeps no resident window and asks for the full range every tick");
     run.late_seconds = 0;
   }
+  if (cpu_ingestor && run.retime_ring) {
+    log.warn("--retime-ring ignored: GPR_INGEST=cpu keeps no resident window and asks for the full range every tick");
+    run.retime_ring = false;
+  }
   std::unique_ptr<gph::WindowSource> src = gph::make_window_source(cli.prometheus_url, ingestor, &log);
   gph::Controller ctl(run, kube.get(), engine.get(), log, gph::system_clock());
   // --snapshot-file: the resident window survives a restart (snapshot.hpp).  The CPU ingest keeps no resident window,
@@ -67,7 +71,7 @@ int main(int argc, char** argv) {
       key.selectors[0] = sel.util, key.selectors[1] = sel.prof, key.selectors[2] = sel.power;
       snapshots = gph::make_file_snapshots(*cli.snapshot_file, key, [ingestor, &cli](std::string* error) {
         return ingestor->resident_session(cli, error);
-      });
+      }, run.retime_ring);
       ctl.use_snapshots(snapshots.get());
     }
   }

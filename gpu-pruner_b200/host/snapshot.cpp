@@ -421,7 +421,7 @@ bool save_snapshot(DeviceIngestSession& session, const SnapshotKey& key, const s
 }
 
 bool restore_snapshot(DeviceIngestSession& session, const SnapshotKey& key, const std::string& path, SnapshotTimes* t,
-                      std::string* why) {
+                      std::string* why, bool retime) {
   const auto t0 = std::chrono::steady_clock::now();
   *t = SnapshotTimes();
   session.invalidate();
@@ -453,8 +453,9 @@ bool restore_snapshot(DeviceIngestSession& session, const SnapshotKey& key, cons
   SnapshotState st;
   ChunkPlaneView planes[2];
   if (!parse_snapshot(reinterpret_cast<const uint8_t*>(buf.data()), n, &have, &st, planes, why, &t->crc_ms)) return false;
-  // taken for another window: the CLI or the window length changed since
-  if (have.span != key.span) {
+  // taken for another window: the CLI or the window length changed since (a shorter window is retimed from a longer
+  // one by the first delta tick when `retime`)
+  if (have.span != key.span && !(retime && have.span > key.span)) {
     *why = "fingerprint mismatch: window of " + std::to_string(have.span) + " s, now " + std::to_string(key.span) + " s";
     return false;
   }
@@ -464,9 +465,19 @@ bool restore_snapshot(DeviceIngestSession& session, const SnapshotKey& key, cons
     *why = b;
     return false;
   }
+  // The selectors end with the window as their range ("[<minutes>m]", promql.cpp render_selectors): a retimed
+  // snapshot's selectors are compared with this run's rendered at the snapshot's window, so every other part must match.
+  const std::string now_range = "[" + std::to_string(key.span / 60) + "m]";
+  const std::string then_range = "[" + std::to_string(have.span / 60) + "m]";
+  auto at_snapshot_window = [&](std::string sel) {
+    if (have.span != key.span && sel.size() >= now_range.size() &&
+        sel.compare(sel.size() - now_range.size(), now_range.size(), now_range) == 0)
+      sel.replace(sel.size() - now_range.size(), now_range.size(), then_range);
+    return sel;
+  };
   static const char* kNames[3] = {"util", "prof", "power"};
   for (int i = 0; i < 3; ++i)
-    if (have.selectors[i] != key.selectors[i]) {
+    if (have.selectors[i] != at_snapshot_window(key.selectors[i])) {
       *why = std::string("fingerprint mismatch: the ") + kNames[i] + " selector changed";
       return false;
     }
@@ -487,8 +498,8 @@ namespace {
 
 class FileSnapshots : public WindowSnapshots {
  public:
-  FileSnapshots(std::string path, SnapshotKey key, std::function<DeviceIngestSession*(std::string*)> session)
-      : path_(std::move(path)), key_(std::move(key)), session_(std::move(session)) {}
+  FileSnapshots(std::string path, SnapshotKey key, std::function<DeviceIngestSession*(std::string*)> session, bool retime)
+      : path_(std::move(path)), key_(std::move(key)), session_(std::move(session)), retime_(retime) {}
 
   bool restore(std::string* line) override {
     std::string err;
@@ -499,7 +510,7 @@ class FileSnapshots : public WindowSnapshots {
     }
     SnapshotTimes t;
     std::string why;
-    if (!restore_snapshot(*s, key_, path_, &t, &why)) {
+    if (!restore_snapshot(*s, key_, path_, &t, &why, retime_)) {
       *line = "Snapshot not restored (" + why + "): starting from the full range";
       return false;
     }
@@ -537,13 +548,15 @@ class FileSnapshots : public WindowSnapshots {
   std::string path_;
   SnapshotKey key_;
   std::function<DeviceIngestSession*(std::string*)> session_;
+  bool retime_;
 };
 
 }  // namespace
 
 std::unique_ptr<WindowSnapshots> make_file_snapshots(std::string path, SnapshotKey key,
-                                                     std::function<DeviceIngestSession*(std::string*)> session) {
-  return std::make_unique<FileSnapshots>(std::move(path), std::move(key), std::move(session));
+                                                     std::function<DeviceIngestSession*(std::string*)> session,
+                                                     bool retime) {
+  return std::make_unique<FileSnapshots>(std::move(path), std::move(key), std::move(session), retime);
 }
 
 }  // namespace gph

@@ -85,13 +85,15 @@ bool parse_snapshot(const uint8_t* buf, size_t n, SnapshotKey* key, SnapshotStat
 bool save_snapshot(DeviceIngestSession& session, const SnapshotKey& key, const std::string& path, SnapshotTimes* t,
                    std::string* error);
 // restore: false = refused, *why says why, and the session is cold (nothing resident).  A snapshot whose key differs
-// from `key` is refused.
+// from `key` is refused — except, with `retime` (--retime-ring), a longer window than key.span: the session is restored
+// at the snapshot's shape and its first delta tick retimes the ring to the shorter window.
 bool restore_snapshot(DeviceIngestSession& session, const SnapshotKey& key, const std::string& path, SnapshotTimes* t,
-                      std::string* why);
+                      std::string* why, bool retime = false);
 
 // The controller's view (controller.hpp WindowSnapshots) of a snapshot file.  `session` returns the ingestor's
 // resident session (nullptr + error: none can be had); it is asked every time, since the engine may replace it.
 std::unique_ptr<WindowSnapshots> make_file_snapshots(std::string path, SnapshotKey key,
-                                                     std::function<DeviceIngestSession*(std::string*)> session);
+                                                     std::function<DeviceIngestSession*(std::string*)> session,
+                                                     bool retime = false);
 
 }  // namespace gph

@@ -318,6 +318,22 @@ GPR_API int gpr_resident_live_rows(gpr_ctx *ctx, uint32_t *bits, int32_t mem_kin
  * reads the re-asked band before and after the tick's merge to see what the late samples changed.           */
 GPR_API int gpr_resident_cols(gpr_ctx *ctx, int32_t plane, uint32_t newer, uint32_t n_cols, float *out,
                               int32_t mem_kind);
+/* Put the ring on a coarser or shorter time grid without a query: keep its newest n_keep buckets and merge them
+ * `factor` to a bucket, newest first, so new bucket b (0 = newest) is the maximum of old buckets
+ * [factor * b, min(factor * b + factor, n_keep)) and n_samples becomes ceil(n_keep / factor).  The merge gives the
+ * bits a fresh gpr_samples_scatter of the same samples gives: every NaN is "no sample", a group without a sample is
+ * the fill 0xFFFFFFFF, +0 beats -0.  A window of N s at step s ending at t_end becomes exactly the window of N' s
+ * at step s' = factor * s ending at t_end when N' <= N and N' % s == 0 (n_keep = N' / s) or N' == N
+ * (n_keep = n_samples); other grids need samples the ring does not hold.  n_pods, n_gpus, the rows and the power
+ * plane stay (power cells are snapped already: a maximum of snapped values is snapped); afterwards
+ * gpr_resident_head reports 0.  With GPR_F_BLOCK_INDEX the index is reallocated for the new n_samples and rebuilt
+ * from the new planes, so it is current after the call even if it was stale before.  Out of place like
+ * gpr_resident_remap: the gathers run on the context's stream after whatever is enqueued there, the call waits for
+ * them, and the peak is the old ring plus the new one in HBM.  Decisions enqueued before the call read the old ring
+ * and retire at the next gpr_sync; pointers from gpr_resident_planes are stale after it.  No resident window is
+ * GPR_E_STATE; factor == 0, n_keep == 0 or n_keep > n_samples GPR_E_INVALID.  On any error (GPR_E_NOMEM included)
+ * the ring, its index and its head are as they were.                                                          */
+GPR_API int gpr_resident_retime(gpr_ctx *ctx, uint32_t n_keep, uint32_t factor);
 
 /* ---- multi-GPU: one process per GPU, pods sharded by rank, one allgather of the bitmap - */
 #define GPR_UNIQUE_ID_BYTES 128
